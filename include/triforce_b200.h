@@ -1,5 +1,5 @@
 /*
- * triforce_b200 — C ABI of the B200-native TriForce hot path (libtriforce_b200.so, sm_100a only).
+ * triforce_b200 — C ABI of the GPU-native TriForce hot path (libtriforce_b200.so, sm_90a / H100 only).
  *
  * The reference (Infini-AI-Lab/TriForce) has no FFI/plugin layer: its hot path crosses into native code only through
  * third-party Python bindings (flash_attn.flash_attn_with_kvcache, ATen ops, NCCL via torch.distributed — SURVEY.md
@@ -30,7 +30,7 @@ typedef void* tf_stream_t; /* cudaStream_t */
 enum {
   TF_OK = 0,
   TF_ERR_INVALID = -1,     /* bad argument (shape, alignment, NULL) */
-  TF_ERR_UNSUPPORTED = -2, /* shape outside what the sm_100a kernels were built for */
+  TF_ERR_UNSUPPORTED = -2, /* shape outside what the sm_90a kernels were built for */
   TF_ERR_WORKSPACE = -3,   /* workspace too small */
   TF_ERR_CUDA = -4         /* a CUDA runtime/driver call failed */
 };
@@ -95,7 +95,7 @@ int tf_rope_append(const void* q, const void* k, const void* v, long long qkv_ro
  * an in-kernel merge by the last CTA of each head.  kv_len = kv_len_host + (kv_len_dev ? *kv_len_dev : 0); `kv_len_max` bounds it (workspace/grid).
  *   q    fp16 [R][H][d] contiguous ; out fp16 [R][H][d] contiguous
  *   k_tensormap / v_tensormap: HOST pointers to descriptors from tf_kv_tensormap_encode (box_keys = TF_VERIFY_BOX_KEYS)
- *   variant: 0 = auto, 1 = mma.sync kernel, 2 = tcgen05/TMEM kernel (not built yet)
+ *   variant: 0 = auto, 1 = mma.sync kernel
  *   clean_keys: keys [0, clean_keys) of this layer are NOT written by the kernels enqueued just before this one (e.g. the
  *              retrieval budget below the gamma+1 fresh slots); with tf_set_pdl the kernel then fills its TMA ring from that
  *              region before `griddepcontrol.wait`.  0 = make no such promise.  Ignored with a device-side length.
@@ -119,15 +119,15 @@ int tf_verify_attn_prefetch(const void* q, const void* k_tensormap, const void* 
                             size_t workspace_bytes, int variant, int clean_keys, const void* next_weights, size_t next_weight_bytes,
                             tf_stream_t stream);
 
-/* tf_tree_attn_tc: the tree (Sequoia) verify attention on the tcgen05 tensor cores — `variant 2` of the verify attention, for
+/* tf_tree_attn_tc: the tree (Sequoia) verify attention on the Hopper tensor cores — `variant 2` of the verify attention, for
  *   R = 128·k query rows (the 512 tree nodes of BASELINE cfg5) against the full KV of one layer; replaces the SDPA call with an
  *   additive [512, S+512] mask at models/tensor_op.py:230-272 / utils/SpecTree_TP.py:168-175.  One CTA = (128-row block, head, KV
- *   split): TMA (SWIZZLE_128B) → S = Q·K^T and O += P·V as tcgen05.mma (M = N = 128, fp16 → fp32 accumulators in TMEM, V consumed
- *   MN-major), softmax rows read with tcgen05.ld, lazy rescale of O in TMEM, tree bitmask as in tf_verify_attn_tree; the splits
- *   are merged by a second small kernel.  Every KV byte is read once per 128-row block (4x for 512 rows) instead of once per
- *   32-row block (16x).  d must be 128; tree_cols = 0 → plain attention over kv_len keys.  causal = 1 (tree_cols = 0): the
- *   bottom-right causal attention of R new rows — the PREFILL attention of a prompt chunk (utils/graph_infer.py:28-37 →
- *   modeling_llama.py:240); tiles above a 256-row block's diagonal are skipped.
+ *   split): TMA (SWIZZLE_128B) → S = Q·K^T and O += P·V as wgmma m64n128k16 (two 64-row warpgroups, fp16 → fp32 accumulators in
+ *   registers, P fed from registers, V consumed MN-major), online softmax in registers, tree bitmask as in tf_verify_attn_tree;
+ *   the splits are merged by a second small kernel.  Every KV byte is read once per 128-row block (4x for 512 rows) instead of
+ *   once per 32-row block (16x).  d must be 128; tree_cols = 0 → plain attention over kv_len keys.  causal = 1 (tree_cols = 0):
+ *   the bottom-right causal attention of R new rows — the PREFILL attention of a prompt chunk (utils/graph_infer.py:28-37 →
+ *   modeling_llama.py:240); tiles above a 128-row block's diagonal are skipped.
  *   `debug_scores`: NULL, or fp32 [128][128] that receives the raw Q·K^T tile of (block 0, head 0, split 0) — test hook.
  */
 size_t tf_tree_attn_tc_workspace_bytes(int R, int H, int kv_len_max);
@@ -136,7 +136,7 @@ int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensor
                     size_t workspace_bytes, float* debug_scores, tf_stream_t stream);
 
 /* Init-time load balancing of tf_verify_attn (no reference counterpart; the reference has no such knob).  The kernel cuts
- * its (head, key-tile) axis into one contiguous range per CTA.  SMs of a B200 do not all pull the same HBM bandwidth, so
+ * its (head, key-tile) axis into one contiguous range per CTA.  Where the SMs of a GPU do not all pull the same HBM bandwidth,
  * an equal cut leaves the kernel waiting for the slowest GPCs; this call measures the per-CTA streaming time of the
  * kernel on the caller's own KV store (R rows over kv_len keys of `layer`; contents are irrelevant) for `rounds`
  * iterations and stores a split table in the workspace, which later launches with the same grid follow.  Results stay

@@ -1,6 +1,6 @@
 # CUDA_VISIBLE_DEVICES=0,1 OMP_NUM_THREADS=48 torchrun --nproc_per_node=2 test/offloading_TP.py --budget 12288 --prefill 130048 --dataset demo --target llama-7B-128K --on_chip 9 --gamma 16
 """The reference's tensor-parallel entry point (same flags and report lines; one process per GPU, NCCL on the o_proj /
-down_proj seams) on the B200-native engine — see `triforce_b200.cli.run_offloading_tp`."""
+down_proj seams) on the GPU-native engine — see `triforce_b200.cli.run_offloading_tp`."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 # CUDA_VISIBLE_DEVICES=0,1 OMP_NUM_THREADS=48 torchrun --nproc_per_node=2 test/offloading_seqouia.py --budget 12288 --prefill 130048 --dataset demo --target llama-7B-128K --on_chip 9 --seed 1
-"""The reference's Sequoia-tree entry point (same flags and report lines) on the B200-native engine — see
+"""The reference's Sequoia-tree entry point (same flags and report lines) on the GPU-native engine — see
 `triforce_b200.cli.run_offloading_seqouia`."""
 import os
 import sys

@@ -1,5 +1,5 @@
 # CUDA_VISIBLE_DEVICES=0 python test/on_chip.py --prefill 124928 --budget 4096 --chunk_size 8 --top_p 0.9 --temp 0.6 --gamma 6 --dataset 128k
-"""The reference's on-chip entry point (same flags and report lines) on the B200-native engine — see
+"""The reference's on-chip entry point (same flags and report lines) on the GPU-native engine — see
 `triforce_b200.cli.run_on_chip`."""
 import os
 import sys

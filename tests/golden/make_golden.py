@@ -13,6 +13,7 @@ Files written:
   forward.npz           reference target forward: last-token logits after a chunked prefill, retrieval-verify logits
   e2e_<cfg>.json        event traces (every sample / rand / Middle_Spec return / target input) of TriForce first and
                         second call (the draft-cache reset quirk, SURVEY §7 hard part 3) and of Autoregressive
+  ref_*                 the reference's PG-19 loader, tree file and command lines (see make_reference_files)
 """
 from __future__ import annotations
 
@@ -241,8 +242,68 @@ def make_tree():
         json.dump(dict(case=case, first_token=first, rounds=rounds), f)
 
 
+def make_reference_files():
+    """Fixtures of the reference's own files, for the CPU tests that compare with them:
+      ref_dataset_gs.npz    `books`: 24 PG-19 books of the reference's data/pg19 (the first 12 rows of each file, text cut to 2000
+                            characters); `lengths` / `ids`: the reference's get_dataset('gs') on them, as one jsonl file, with the
+                            byte tokenizer of tests/test_dataset_cpu.py
+      ref_tree_512.npz      the reference's tree/512.pt (lists as JSON, the mask bit-packed)
+      ref_cli_flags.json    every add_argument flag of the reference's test/{on_chip,offloading_TP,offloading_seqouia}.py with its default
+    """
+    import importlib.util
+    import re
+    import shutil
+    import tempfile
+
+    books = []
+    for name in ("pg19-test.json", "pg19-train.json"):
+        with open(os.path.join(rh.REF_ROOT, "data", "pg19", name), encoding="utf-8") as f:
+            rows = [json.loads(line) for line in f if line.strip()][:12]
+        books += [{"text": r["text"][:2000]} for r in rows]
+
+    from test_dataset_cpu import ByteTokenizer
+    tmp = tempfile.mkdtemp()
+    try:
+        os.environ.update(HF_HOME=os.path.join(tmp, "hf"), HF_DATASETS_CACHE=os.path.join(tmp, "hf", "datasets"), HF_DATASETS_OFFLINE="1")
+        os.makedirs(os.path.join(tmp, "data", "pg19"))
+        with open(os.path.join(tmp, "data", "pg19", "sample.jsonl"), "w", encoding="utf-8") as f:
+            for b in books:
+                f.write(json.dumps(b) + "\n")
+        spec = importlib.util.spec_from_file_location("ref_dataset", os.path.join(rh.REF_ROOT, "data", "dataset.py"))
+        ref = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(ref)
+        cwd = os.getcwd()
+        os.chdir(tmp)  # the reference opens "data/pg19/" relative to the working directory
+        try:
+            gs = ref.get_dataset("gs", tokenizer=ByteTokenizer())
+        finally:
+            os.chdir(cwd)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    np.savez_compressed(os.path.join(HERE, "ref_dataset_gs.npz"), books=np.array([b["text"] for b in books]), lengths=np.array([t.shape[-1] for t in gs], np.int64),
+                        ids=np.concatenate([t.reshape(-1).numpy() for t in gs]).astype(np.int32))
+    print(f"[reference files] get_dataset('gs'): {len(gs)} prompts")
+
+    g = torch.load(os.path.join(rh.REF_ROOT, "tree", "512.pt"), weights_only=False)
+    lists = {k: g[k] for k in ("roots", "branches", "Successors", "size")}
+    np.savez_compressed(os.path.join(HERE, "ref_tree_512.npz"), lists=np.array(json.dumps(lists)),
+                        mask=np.packbits(g["mask"].numpy() != 0, axis=1), depth=g["depth"].numpy())
+
+    flags = {}
+    for entry in ("on_chip", "offloading_TP", "offloading_seqouia"):
+        with open(os.path.join(rh.REF_ROOT, "test", entry + ".py")) as f:
+            src = f.read()
+        flags[entry] = {}
+        for flag, rest in re.findall(r"add_argument\('--(\w+)'(.*?)\)\n", src):
+            m = re.search(r"default=([^,)]+)", rest)
+            flags[entry][flag] = (m.group(1).strip().strip("'").strip('"') if m else
+                                  "store_true" if "store_true" in rest else None)
+    with open(os.path.join(HERE, "ref_cli_flags.json"), "w") as f:
+        json.dump(flags, f, indent=1)
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["retrieval", "sampling", "forward", "e2e", "tree"]
+    which = sys.argv[1:] or ["retrieval", "sampling", "forward", "e2e", "tree", "reference_files"]
     with torch.inference_mode():
         if "retrieval" in which:
             make_retrieval_build()
@@ -254,3 +315,5 @@ if __name__ == "__main__":
             make_e2e()
         if "tree" in which:
             make_tree()
+        if "reference_files" in which:
+            make_reference_files()

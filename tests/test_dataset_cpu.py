@@ -1,5 +1,5 @@
-"""Input pipeline (SURVEY §8 row f-4): `data.dataset.get_dataset` against hand-made jsonl books and — in the build container, where
-the reference checkout and the `datasets` package exist — against the reference's own `get_dataset` on its own PG-19 files."""
+"""Input pipeline (SURVEY §8 row f-4): `data.dataset.get_dataset` against hand-made jsonl books and against the reference's own
+`get_dataset` on a stored sample of its PG-19 files (tests/golden/ref_dataset_gs.npz)."""
 import json
 import os
 import sys
@@ -61,30 +61,16 @@ def test_lwm_chat_wrapper_truncates_and_wraps():
     assert text.endswith("ASSISTANT: ")
 
 
-_REF_CHILD = r"""
-import importlib.util, os, sys, torch
-sys.path.insert(0, os.path.join(sys.argv[1], "tests"))
-from test_dataset_cpu import ByteTokenizer
-spec = importlib.util.spec_from_file_location("ref_dataset", "/root/reference/data/dataset.py")
-ref = importlib.util.module_from_spec(spec)
-spec.loader.exec_module(ref)
-os.chdir("/root/reference")  # the reference opens "data/pg19/" relative to the working directory
-torch.save(ref.get_dataset("gs", tokenizer=ByteTokenizer()), sys.argv[2])
-"""
-
-
-@pytest.mark.skipif(not os.path.isdir("/root/reference/data/pg19"), reason="reference checkout not on this box")
-def test_against_the_reference_get_dataset(tmp_path):
-    """The reference's own get_dataset('gs') on its own PG-19 files, run in a child process whose HF caches point into tmp_path."""
-    pytest.importorskip("datasets")
-    import subprocess
-    out = tmp_path / "ref_gs.pt"
-    env = dict(os.environ, HF_HOME=str(tmp_path / "hf"), HF_DATASETS_CACHE=str(tmp_path / "hf" / "datasets"), HF_DATASETS_OFFLINE="1")
-    r = subprocess.run([sys.executable, "-c", _REF_CHILD, REPO, str(out)], capture_output=True, text=True, timeout=600, env=env)
-    if r.returncode != 0 or not out.exists():
-        pytest.skip(f"reference get_dataset did not run here: {r.stderr[-300:]}")
-    want = torch.load(out)
-    got = get_dataset("gs", ByteTokenizer(), root="/root/reference/data/pg19")
+def test_against_the_reference_get_dataset(golden_dir, tmp_path):
+    """The reference's own get_dataset('gs') (stored by tests/golden/make_golden.py) on a sample of its PG-19 files."""
+    import numpy as np
+    ref = np.load(os.path.join(golden_dir, "ref_dataset_gs.npz"))
+    with open(tmp_path / "sample.jsonl", "w", encoding="utf-8") as f:
+        for text in ref["books"]:
+            f.write(json.dumps({"text": str(text)}) + "\n")
+    want = np.split(ref["ids"].astype(np.int64), np.cumsum(ref["lengths"])[:-1])
+    got = get_dataset("gs", ByteTokenizer(), root=str(tmp_path))
     assert len(got) == len(want) == 20
     for a, b in zip(got, want):
-        assert torch.equal(a, b)
+        assert a.dtype == torch.long and a.shape == (1, len(b))
+        assert torch.equal(a[0], torch.from_numpy(b))

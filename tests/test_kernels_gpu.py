@@ -1,4 +1,4 @@
-"""GPU parity tests: every sm_100a kernel, called THROUGH THE C ABI (triforce_b200.ops → ctypes), against the CPU oracle
+"""GPU parity tests: every sm_90a kernel, called THROUGH THE C ABI (triforce_b200.ops → ctypes), against the CPU oracle
 on the same seeded inputs.  Bit-exact for index / byte / fp16-elementwise work, stated tolerances for attention."""
 import os
 
@@ -836,8 +836,8 @@ def test_verify_attn_tree_matches_oracle(R, H, d, S, T, row0):
 
 @pytest.mark.parametrize("R,H,S,T", [(128, 2, 1000, 0), (128, 3, 1024 + 128, 128), (256, 2, 3000, 256), (512, 2, 5000 + 512, 512), (128, 1, 128, 0)])
 def test_tree_attn_tcgen05_matches_oracle(R, H, S, T):
-    """The tcgen05 / TMEM tree-verify kernel (variant 2) against the oracle's attention_tree, and its raw first score tile
-    against an fp32 Q·K^T (which checks the UMMA shared-memory / instruction descriptors in isolation)."""
+    """The wgmma tree-verify kernel (variant 2) against the oracle's attention_tree, and its raw first score tile
+    against an fp32 Q·K^T (which checks the wgmma shared-memory descriptors in isolation)."""
     d = 128
     rng = np.random.Generator(np.random.PCG64(S + R + T))
     q = rng.standard_normal((R, H, d), dtype=np.float32).astype(np.float16)
@@ -862,7 +862,7 @@ def test_tree_attn_tcgen05_matches_oracle(R, H, S, T):
 
 @pytest.mark.parametrize("R,H,S", [(128, 2, 128), (128, 2, 1000), (1024, 2, 1024), (1024, 2, 3000), (1023, 1, 2500), (200, 3, 777), (40, 2, 333)])
 def test_prefill_attention_tcgen05_causal_matches_oracle(R, H, S):
-    """Causal mode of the tcgen05 kernel = the prefill attention of a prompt chunk (row i sees keys <= S - R + i), any R."""
+    """Causal mode of the wgmma kernel = the prefill attention of a prompt chunk (row i sees keys <= S - R + i), any R."""
     d = 128
     rng = np.random.Generator(np.random.PCG64(S * 7 + R))
     q = rng.standard_normal((R, H, d), dtype=np.float32).astype(np.float16)

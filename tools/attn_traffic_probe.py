@@ -24,7 +24,7 @@ def main():
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
     S, R, H, d = args.kv_len, args.rows, args.heads, args.head_dim
-    L = 2  # alternate two layers so that no launch finds its keys in the 126 MB L2
+    L = 2  # alternate two layers so that no launch finds its keys in the 50 MB L2
     Ks = torch.randn((L, H, S + 64, d), device=dev, dtype=torch.float16)
     Vs = torch.randn((L, H, S + 64, d), device=dev, dtype=torch.float16)
     q = torch.randn((R, H, d), device=dev, dtype=torch.float16)

@@ -123,7 +123,6 @@ def lib() -> ctypes.CDLL:
     _lib = L
     # programmatic dependent launch mask of the decode-path kernels (tf_set_pdl): on by default for every kernel of the chain
     # (1 add_rmsnorm, 2 silu_mul, 4 rope_append, 8 draft_attn, 16 verify_attn on short stores, 32 skinny_gemm, 128 stream_linear, 256 the one-shot peer all-reduce);
-    # measured on B200: retrieval verify 3.81 -> 3.43 ms, full-KV step 12.4 -> 11.9 ms (profiles/r02_profile_step_pdl.md)
     L.tf_set_pdl(int(os.environ.get("TRIFORCE_PDL", str(DEFAULT_PDL_MASK))))
     return L
 

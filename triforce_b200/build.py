@@ -1,4 +1,4 @@
-"""Builds libtriforce_b200.so (sm_100a only) in-tree with nvcc, and the C oracle helpers are not part of it.
+"""Builds libtriforce_b200.so (sm_90a, H100) in-tree with nvcc, and the C oracle helpers are not part of it.
 
     python -m triforce_b200.build            # build if stale
     python -m triforce_b200.build --force
@@ -19,7 +19,7 @@ STAMP = os.path.join(LIB_DIR, "build.stamp")
 
 SOURCES = ["abi.cu", "retrieval_build.cu", "verify_attn.cu", "decoder_ops.cu", "sampling.cu", "skinny_gemm.cu", "stream_linear.cu", "tree_attn_tc.cu", "allreduce.cu", "loop_graph.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "--use_fast_math=false",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "--use_fast_math=false",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "--extended-lambda",
     "-Xptxas", "-v",
 ]

@@ -1,6 +1,6 @@
 """KV caches of the TriForce hierarchy — same classes, constructor arguments, attributes and method names as the
 reference's `models/cache.py` (FlashSimpleCache :20-61, RetrievalCache :117-198, StreamingLLMEvictionCache :200-265),
-re-laid-out for B200.
+re-laid-out for the GPU kernels.
 
 Physical layout is HEAD-MAJOR `[L, H, slots, d]` fp16: one (layer, head) stream is contiguous, so the verify kernel's
 TMA boxes are dense 128-byte rows and an 8-token retrieval chunk is one contiguous 2 KB block.  `.key_cache` /

@@ -1,10 +1,10 @@
 """Command-line front ends behind the reference's three entry points (`test/on_chip.py`, `test/offloading_TP.py`,
 `test/offloading_seqouia.py`): the same flags with the same defaults, the same measurement flow and report lines, on the
-B200-native engine.  The scripts under `test/` are one-line wrappers around the `run_*` functions here.
+GPU-native engine.  The scripts under `test/` are one-line wrappers around the `run_*` functions here.
 
 Offline by design (no HF hub, no tokenizer, no dataset files on the box): models are random-init with the named shapes
 unless `--target_path` / `--draft_path` point at local HF checkpoints, and the prompt is synthetic token ids.
-`--on_chip` of the TP scripts is accepted and ignored — a B200 keeps the whole KV in HBM.
+`--on_chip` of the TP scripts is accepted and ignored — the engine keeps the whole KV in HBM.
 """
 from __future__ import annotations
 

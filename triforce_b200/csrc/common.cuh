@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of libtriforce_b200.so.
+// Shared helpers for the sm_90a kernels of libtriforce_b200.so.
 #pragma once
 
 #include <cuda.h>

@@ -243,7 +243,7 @@ int tf_retrieval_build(const void* K, const void* V, long long kv_layer_stride, 
     if (!idx) idx = (int32_t*)(ws + align_up((size_t)n_layers * H * chunks * sizeof(__half), 256));
   }
 
-  const int sms = sm_count() > 0 ? sm_count() : 148;
+  const int sms = sm_count() > 0 ? sm_count() : 132;
   {
     const int per_pass = 32 / (d / 8);
     const int passes = (chunks + per_pass - 1) / per_pass;

@@ -109,8 +109,8 @@ __device__ __forceinline__ ArgBest block_argmax(ArgBest b, float* redv, int* red
 }
 
 // IEEE division out of line: the correctly rounded quotient the reference's `/` gives (ATen), without replicating the
-// special-case path of div.rn at every unrolled call site — the 25 K-instruction norm_logits body spent 27 % of its issue slots
-// waiting for instructions (ncu: stall_no_inst, profiles/r02_sampling_kernels.md).
+// special-case path of div.rn at every unrolled call site, which would bloat the 25 K-instruction norm_logits body and stall
+// it on instruction fetch.
 __device__ __noinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
 
 // argmax_i num(i) / expo[i] over [0,V); every thread returns the winner.  Eight independent iterations in flight per thread.

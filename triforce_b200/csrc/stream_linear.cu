@@ -542,7 +542,7 @@ int tf_weight_tensormap_encode(void* out, const void* W, int N, int K, long long
 
 size_t tf_stream_linear_workspace_bytes(void) {
   int sms = tf::sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   return (size_t)(2 * sms + 1) * (3 * 32 * sizeof(float4) + sizeof(int)) + 256;
 }
 
@@ -569,7 +569,7 @@ static int stream_linear_impl(const void* x, long long x_row_stride, const void*
   if (peers) a.peers = *peers;
   const int tiles = epilogue == 1 ? (N / 2 + 7) / 8 : (N + kSlRows - 1) / kSlRows;
   int sms = sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   const int want = plan.ctas_per_sm * sms;
   const int grid = tiles < want ? tiles : want;
   a.part = (float4*)workspace;

@@ -1,28 +1,25 @@
-// Tree (Sequoia) verify attention on the 5th-generation tensor cores: R = 128·k query rows (the 512 tree nodes of BASELINE
+// Tree (Sequoia) verify attention on the Hopper tensor cores (wgmma): R = 128·k query rows (the 512 tree nodes of BASELINE
 // cfg5) against the full KV of one layer — `variant = 2` of tf_verify_attn_tree.  Replaces the SDPA-with-additive-mask call of
 // the reference (models/tensor_op.py:230-272 → F.scaled_dot_product_attention with a [512, S+512] fp16 mask, 134 MB at 128K).
 // The same kernel in CAUSAL mode is the prefill attention (SURVEY §8 row f-2): the R rows of a prompt chunk against the keys
 // written so far, bottom-right causal — the reference's eager 128-token chunks through flash_attn_with_kvcache
 // (utils/graph_infer.py:28-37 → models/modeling_llama.py:240); tiles above a block's diagonal are never loaded.
 //
-// This is the one place in the hot path where the (rows x d) x (d x keys) contraction FILLS a tensor-core tile: 512 rows give
-// 2·512 FLOP per KV byte (ridge of a B200 ≈ 218 FLOP/B), i.e. the launch is tensor-bound — 2·2·512·S·H·d FLOP per layer
-// (13B @ 131 584 keys: 1.38 TFLOP) — where the mma.sync kernel had to re-read the KV once per 32-row block (16 passes).
+// This is the one place in the hot path where the (rows x d) x (d x keys) contraction FILLS a tensor-core tile: each KV byte
+// feeds 128 query rows of a CTA (2·128 FLOP per byte; the other row blocks of the same head read it from L2), where the
+// mma.sync kernel had to re-read the KV once per 32-row block.
 //
-// One CTA = (128-row query block, head, KV split).  Warp roles (256 threads):
-//   warp 0  TMA producer: Q block once (tensor map over [R][H][d]), then K and V tiles of 128 keys (four 64x64 boxes each,
-//           SWIZZLE_128B — exactly the canonical K-major / MN-major UMMA shared-memory layouts) into a 5-slot mbarrier ring
-//           of single tiles (K0 V0 K1 V1 ...: a K slot is released by the QK^T that read it, a V slot by its PV);
-//   warp 1  MMA issuer (one elected lane): S = Q·K^T  (tcgen05.mma kind::f16, M = 128, N = 128, 8 x K = 16; A, B K-major)
-//           into one of two 128-column TMEM accumulators, and O += P·V (A = P from shared memory, K-major; B = V MN-major)
-//           into a third; completion is signalled with tcgen05.commit on mbarriers;
-//   warp 2  TMEM allocation / release (512 columns);
-//   warps 4-7  softmax: thread r owns query row r = TMEM lane r.  Two passes over the score row with tcgen05.ld (max, then
-//           exp2 / sum / fp16 pack), P written to shared memory in the swizzled K-major layout the MMA reads, O rescaled in
-//           TMEM (tcgen05.ld → scale → tcgen05.st) only when the running maximum moved by more than 2^8 (lazy rescale);
-//           the tree mask (ancestor bitmask of the last T columns) and the kv_len bound are applied to the tiles they touch.
-//   QK^T of tile j+1 is issued before the softmax of tile j finishes (two S accumulators), so tensor cores and the MUFU /
-//   FMA pipes overlap.
+// One CTA = (128-row query block, head, KV split), 288 threads:
+//   warps 0-7  two consumer warpgroups; warpgroup w owns query rows 64w .. 64w+63 of the block.  Per 128-key tile:
+//              S = Q·K^T as 8 x wgmma m64n128k16 (A = Q, B = K, both K-major from shared memory) into 64 fp32 registers per
+//              thread, online softmax in registers (quad shuffles for the row maximum, exp2 domain), P packed to fp16 in
+//              registers in exactly the A-fragment layout of the next wgmma, O += P·V as 8 x wgmma m64n128k16 with A from
+//              registers and B = V MN-major (transposed) from shared memory; the tree mask (ancestor bitmask of the last T
+//              columns), the kv_len bound and the causal diagonal are applied to the tiles they touch.
+//   warp 8     TMA producer: the Q block once (tensor map over [R][H][d]), then K and V tiles of 128 keys (four 64x64 boxes
+//              each, SWIZZLE_128B — exactly the canonical K-major / MN-major wgmma shared-memory layouts) into a ring of single
+//              32 KB tiles in the order K0 V0 K1 V1 ...; a slot is released when both warpgroups' wgmmas that read it completed.
+//   The two warpgroups are independent: while one runs its softmax, the tensor core serves the other's wgmmas.
 // Partials (m, l, unnormalised O) per (block, head, split) go to the workspace; `tree_attn_merge_kernel` combines the splits.
 #include <string.h>
 
@@ -30,79 +27,59 @@
 
 namespace tf {
 
-constexpr int kTcRows = 128;          // query rows per CTA (UMMA M)
-constexpr int kTcKeys = 128;          // keys per tile (UMMA N of QK^T, K extent of PV)
-constexpr int kTcD = 128;             // head dim
-constexpr int kTcBlockRows = 256;      // query rows per CTA: two UMMA tiles sharing every K / V tile
-constexpr int kTcSlots = 3;            // ring of single 32 KB K / V tiles (load order K0 K1 V0 K2 V1 ...)
-constexpr int kTcThreads = 384;
-constexpr uint32_t kTcTileBytes = kTcKeys * kTcD * 2;  // 32 KB: one K or V tile, also the Q block and the P tile
+constexpr int kTcKeys = 128;           // keys per tile (wgmma N of QK^T, K extent of PV)
+constexpr int kTcD = 128;              // head dim
+constexpr int kTcBlockRows = 128;      // query rows per CTA: two 64-row warpgroups sharing every K / V tile
+constexpr int kTcSlots = 4;            // ring of single 32 KB K / V tiles (two tiles of keys in flight)
+constexpr int kTcConsumerWarps = 8;
+constexpr int kTcThreads = (kTcConsumerWarps + 1) * 32;
+constexpr uint32_t kTcTileBytes = kTcKeys * kTcD * 2;  // 32 KB: one K or V tile, also the Q block
 constexpr uint32_t kTcHalfBytes = kTcTileBytes / 2;    // one 64-element (128-byte) column half: 128 rows x 128 B
-constexpr float kTcLazyLog2 = 8.f;
 
-// ---- tcgen05 wrappers -------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_alloc(uint32_t* slot_in_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// ---- wgmma wrappers ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+#define TC_ACC8(x, i) "+f"(x[i]), "+f"(x[i + 1]), "+f"(x[i + 2]), "+f"(x[i + 3]), "+f"(x[i + 4]), "+f"(x[i + 5]), "+f"(x[i + 6]), "+f"(x[i + 7])
+#define TC_ACC64(x) TC_ACC8(x, 0), TC_ACC8(x, 8), TC_ACC8(x, 16), TC_ACC8(x, 24), TC_ACC8(x, 32), TC_ACC8(x, 40), TC_ACC8(x, 48), TC_ACC8(x, 56)
+#define TC_D64 \
+  "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,"  \
+  "%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+
+// d[64x128] (+)= A[64x16] · B[16x128], A and B from shared memory, both K-major
+__device__ __forceinline__ void wg_mma_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " TC_D64 ", %64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : TC_ACC64(d)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {  // arrives on `bar` when all MMAs issued so far have completed
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {  // this warp's 32 lanes x 32 consecutive columns
+// d[64x128] += A[64x16] · B[16x128], A from registers (the m64k16 A fragment), B from shared memory MN-major (transposed)
+__device__ __forceinline__ void wg_mma_rs_tb(float (&d)[64], const uint32_t* a, uint64_t bdesc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
-      "%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-        "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-        "=r"(v[31])
-      : "r"(taddr)
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " TC_D64 ", {%64,%65,%66,%67}, %68, 1, 1, 1, 1;\n"
+      : TC_ACC64(d)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
       : "memory");
 }
-__device__ __forceinline__ void tc_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
-      "%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]),
-      "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]),
-      "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory descriptors (cute/arch/mma_sm100_desc.hpp: SmemDescriptor).  Both describe a [128 rows][64 fp16] half
-// tile of 128-byte rows under SWIZZLE_128B (8-row atoms of 1024 B), as TMA writes it:
+// wgmma shared-memory descriptor (cute/arch/mma_sm90_desc.hpp: GmmaDescriptor) of a [rows][64 fp16] half tile of 128-byte rows
+// under SWIZZLE_128B (8-row atoms of 1024 B), as TMA writes it:
 //   K-major (the contraction runs along the 128-byte row): SBO = 1024 B between 8-row groups; a K = 16 step = +32 B;
-//   MN-major (the row IS the M/N extent, contraction across rows): LBO = distance to the next 64-element half (16 KB),
+//   MN-major (the row IS the N extent, contraction across rows): LBO = distance to the next 64-element half (16 KB),
 //   SBO = 1024 B between 8-row (= 8-k) groups; a K = 16 step = +16 rows = +2048 B.
-__device__ __forceinline__ uint64_t tc_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;  // LayoutType::SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // LayoutType::B128 (SWIZZLE_128B)
   return d;
-}
-// Instruction descriptor (UMMA::InstrDescriptor): D fp32, A / B fp16, M = 128, N = 128, optional MN-major B
-__host__ __device__ constexpr uint32_t tc_idesc(bool b_mn_major) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((b_mn_major ? 1u : 0u) << 16) | ((uint32_t)(kTcKeys >> 3) << 17) | ((uint32_t)(kTcRows >> 4) << 24);
 }
 
 __device__ __forceinline__ void tc_tma_3d(uint32_t smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
@@ -120,9 +97,9 @@ struct TcArgs {
   int causal;                 // 1: bottom-right causal mask of R new rows (prefill chunks): row i sees key j iff j <= kv_len - R + i
   float scale_log2;
   int splits, tiles_per_split;
-  float* part_o;              // [blocks][H][splits][256][128] unnormalised
-  float* part_m;              // [blocks][H][splits][256]   running maximum (log2 domain), -inf when the split saw nothing
-  float* part_l;              // [blocks][H][splits][256]
+  float* part_o;              // [blocks][H][splits][128][128] unnormalised
+  float* part_m;              // [blocks][H][splits][128]   running maximum (log2 domain), -inf when the split saw nothing
+  float* part_l;              // [blocks][H][splits][128]
   float* debug_s;             // nullable: scores of the CTA's first tile (block 0, head 0, split 0, rows 0..127) — test hook
 };
 
@@ -148,26 +125,26 @@ __device__ __forceinline__ float tc_ex2(float x) {
   return y;
 }
 
-// One CTA = (256-row query block = two 128-row UMMA tiles, head, KV split).  384 threads:
-//   warp 0 TMA, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-7 softmax of query tile 0, warps 8-11 softmax of tile 1.
-// TMEM columns: S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512).  Both query tiles share every K / V tile (each KV byte is
-// read once per 256 rows), and while one softmax group works on its score tile the tensor core runs the other group's MMAs.
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+  const __half2 h = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// Register fragments (wgmma m64nNk16, per warp of the warpgroup: 16 rows; g = lane / 4, t = lane % 4):
+//   accumulator element 4n + e  <->  row g + 8 (e >> 1), column 8n + 2t + (e & 1)
+//   A fragment of k-step kk     <->  {row g, keys 16kk + 2t..}, {row g+8, same}, {row g, keys 16kk + 8 + 2t..}, {row g+8, same}
+// so the scores of keys 16kk .. 16kk+15 (accumulator elements 8kk .. 8kk+7) are, packed in pairs, the A fragment of PV step kk.
 __global__ void __launch_bounds__(kTcThreads, 1)
     tree_attn_tc_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant__ CUtensorMap kmap, const __grid_constant__ CUtensorMap vmap,
                         const TcArgs a) {
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* q_s = smem;                                  // [2 tiles][2 halves][128 rows][128 B]
-  uint8_t* p_s = q_s + 2 * kTcTileBytes;                // same layout, fp16 probabilities of the two tiles
-  uint8_t* kv_s = p_s + 2 * kTcTileBytes;               // [slots] single tiles: K0 V0 K1 V1 ...
+  uint8_t* q_s = smem;                      // [2 halves][128 rows][128 B]
+  uint8_t* kv_s = q_s + kTcTileBytes;       // [slots] single tiles [2 halves][128 keys][128 B]: K0 V0 K1 V1 ...
   uint64_t* bars = reinterpret_cast<uint64_t*>(kv_s + (size_t)kTcSlots * kTcTileBytes);
   uint64_t* q_full = bars;                  // 1
   uint64_t* kv_full = bars + 1;             // [slots]
   uint64_t* kv_empty = kv_full + kTcSlots;  // [slots]
-  uint64_t* s_full = kv_empty + kTcSlots;   // [2]  scores of query tile g are in TMEM
-  uint64_t* p_full = s_full + 2;            // [2]  probabilities of query tile g are in shared memory (and S_g is free)
-  uint64_t* o_done = p_full + 2;            // [2]  PV of query tile g has completed (O_g updated, P_g free)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qb = blockIdx.x, h = blockIdx.y, sp = blockIdx.z;
@@ -182,39 +159,27 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < kTcSlots; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int g = 0; g < 2; ++g) { mbar_init(&s_full[g], 1); mbar_init(&p_full[g], 128); mbar_init(&o_done[g], 1); }
+    for (int s = 0; s < kTcSlots; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], kTcConsumerWarps); }
     fence_mbar_init();
   }
-  if (warp == 2) tc_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;  // base (lane 0, column 0) of the allocation
 
-  if (warp == 0) {
+  if (warp == kTcConsumerWarps) {
     // ================= TMA producer =================
     if (lane == 0 && n_tiles > 0) {
       prefetch_tensormap(&qmap);
       prefetch_tensormap(&kmap);
       prefetch_tensormap(&vmap);
-      mbar_expect_tx(q_full, 2 * kTcTileBytes);
-#pragma unroll
-      for (int g = 0; g < 2; ++g) {  // rows beyond R are zero-filled by TMA (their results are never stored)
-        tc_tma_3d(smem_u32(q_s) + g * kTcTileBytes, &qmap, q_full, 0, h, qb * kTcBlockRows + g * kTcRows);
-        tc_tma_3d(smem_u32(q_s) + g * kTcTileBytes + kTcHalfBytes, &qmap, q_full, 64, h, qb * kTcBlockRows + g * kTcRows);
-      }
-      // load order K0 K1 V0 K2 V1 K3 V2 ... V(n-1): K runs one tile ahead of V, so that with only three 32 KB slots every load is
-      // issued about one whole tile period before its consumer needs it (item i reuses the slot of item i-3)
+      mbar_expect_tx(q_full, kTcTileBytes);  // rows beyond R are zero-filled by TMA (their results are never stored)
+      tc_tma_3d(smem_u32(q_s), &qmap, q_full, 0, h, qb * kTcBlockRows);
+      tc_tma_3d(smem_u32(q_s) + kTcHalfBytes, &qmap, q_full, 64, h, qb * kTcBlockRows);
       for (int i = 0; i < 2 * n_tiles; ++i) {
-        const bool is_v = (i == 2 * n_tiles - 1) || (i >= 2 && (i & 1) == 0);
-        const int tile = (i == 2 * n_tiles - 1) ? n_tiles - 1 : (i == 0 ? 0 : ((i & 1) ? (i + 1) / 2 : i / 2 - 1));
         const uint32_t s = (uint32_t)i % kTcSlots, ph = ((uint32_t)i / kTcSlots) & 1u;
         mbar_wait(&kv_empty[s], ph ^ 1u);
         mbar_expect_tx(&kv_full[s], kTcTileBytes);
-        const int key0 = (t_begin + tile) * kTcKeys;
+        const int key0 = (t_begin + (i >> 1)) * kTcKeys;
         uint8_t* dst = kv_s + (size_t)s * kTcTileBytes;
-        const CUtensorMap* map = is_v ? &vmap : &kmap;
+        const CUtensorMap* map = (i & 1) ? &vmap : &kmap;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
 #pragma unroll
@@ -223,201 +188,132 @@ __global__ void __launch_bounds__(kTcThreads, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0 && n_tiles > 0) {
-      constexpr uint32_t idesc_qk = tc_idesc(false), idesc_pv = tc_idesc(true);
-      const uint32_t q_u = smem_u32(q_s), p_u = smem_u32(p_s);
-      auto k_item = [&](int j) { return (uint32_t)(j == 0 ? 0 : 2 * j - 1); };                          // position in the load order
-      auto v_item = [&](int j) { return (uint32_t)(j == n_tiles - 1 ? 2 * n_tiles - 1 : 2 * j + 2); };
-      auto k_slot = [&](int j) { return k_item(j) % kTcSlots; };
-      auto v_slot = [&](int j) { return v_item(j) % kTcSlots; };
-      auto issue_qk = [&](int g, int j) {  // S_g = Q_g K_j^T (the K tile must have landed)
-        const uint32_t k_u = smem_u32(kv_s + (size_t)k_slot(j) * kTcTileBytes);
-        const uint32_t acc = tmem + (uint32_t)g * 128u;
+    return;
+  }
+
+  // ================= consumer warpgroups =================
+  const int wg = warp >> 2;                         // 64-row half of the block
+  const int g = lane >> 2, t = lane & 3;
+  const int rb0 = wg * 64 + (warp & 3) * 16 + g;    // rows of this thread within the block: rb0 and rb0 + 8
+  const int row0 = qb * kTcBlockRows + rb0;
+  const int prefix = a.kv_len - a.tree_cols;
+  const int words = a.tree_cols >> 5;
+  const uint32_t* mrow[2] = {a.tree_mask != nullptr ? a.tree_mask + (size_t)min(row0, a.R - 1) * words : nullptr,
+                             a.tree_mask != nullptr ? a.tree_mask + (size_t)min(row0 + 8, a.R - 1) * words : nullptr};
+  const uint32_t q_u = smem_u32(q_s) + (uint32_t)wg * 64u * 128u;
+  float o[64];
 #pragma unroll
-        for (int kk = 0; kk < kTcD / 16; ++kk) {
-          const uint32_t off = (uint32_t)(kk >> 2) * kTcHalfBytes + (uint32_t)(kk & 3) * 32u;
-          tc_mma_f16(acc, tc_desc(q_u + (uint32_t)g * kTcTileBytes + off, 16, 1024), tc_desc(k_u + off, 16, 1024), idesc_qk, kk > 0 ? 1u : 0u);
-        }
-        tc_commit(&s_full[g]);
-      };
-      auto issue_pv = [&](int g, int j) {  // O_g += P_g V_j
-        const uint32_t v_u = smem_u32(kv_s + (size_t)v_slot(j) * kTcTileBytes);
-        const uint32_t acc = tmem + 256u + (uint32_t)g * 128u;
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // running maximum (log2 domain, scaled) and partial denominator
+
+  if (n_tiles > 0) mbar_wait(q_full, 0);
+  for (int j = 0; j < n_tiles; ++j) {
+    const uint32_t ks = (uint32_t)(2 * j) % kTcSlots, kph = ((uint32_t)(2 * j) / kTcSlots) & 1u;
+    const uint32_t vs = (uint32_t)(2 * j + 1) % kTcSlots, vph = ((uint32_t)(2 * j + 1) / kTcSlots) & 1u;
+    const int key0 = (t_begin + j) * kTcKeys;
+    // ---- S = Q K^T ----
+    float s[64];
+    mbar_wait(&kv_full[ks], kph);
+    const uint32_t k_u = smem_u32(kv_s + (size_t)ks * kTcTileBytes);
+    wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < kTcKeys / 16; ++kk) {
-          // A = P_g [128 rows][128 keys] K-major: key step kk → half kk/4, +32 B per step inside the half
-          const uint32_t a_off = (uint32_t)g * kTcTileBytes + (uint32_t)(kk >> 2) * kTcHalfBytes + (uint32_t)(kk & 3) * 32u;
-          // B = V [128 keys][128 d] MN-major: 16 keys = 16 rows of 128 B; the two d halves are LBO = 16 KB apart
-          const uint32_t b_off = (uint32_t)kk * 16u * 128u;
-          tc_mma_f16(acc, tc_desc(p_u + a_off, 16, 1024), tc_desc(v_u + b_off, kTcHalfBytes, 1024), idesc_pv, (j > 0 || kk > 0) ? 1u : 0u);
+    for (int kk = 0; kk < kTcD / 16; ++kk) {
+      const uint32_t off = (uint32_t)(kk >> 2) * kTcHalfBytes + (uint32_t)(kk & 3) * 32u;
+      wg_mma_ss(s, wg_desc(q_u + off, 16, 1024), wg_desc(k_u + off, 16, 1024), kk > 0 ? 1u : 0u);
+    }
+    wg_commit();
+    wg_wait_all();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[ks]);
+    if (a.debug_s != nullptr && j == 0 && qb == 0 && h == 0 && sp == 0) {  // test hook: the raw score tile
+#pragma unroll
+      for (int i = 0; i < 64; ++i) a.debug_s[(size_t)(rb0 + 8 * ((i >> 1) & 1)) * 128 + 8 * (i >> 2) + 2 * t + (i & 1)] = s[i];
+    }
+    // does this tile touch tree columns / the end of the keys / (causal) the diagonal of this block?  (uniform per CTA)
+    const bool masked_tile = a.causal ? key0 + kTcKeys - 1 > a.kv_len - a.R + qb * kTcBlockRows : key0 + kTcKeys > prefix;
+    if (masked_tile) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        uint32_t vis[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          if (a.causal) {  // keys key0+32c .. : visible up to lim = min(kv_len - 1, kv_len - R + row)
+            const int nvis = min(a.kv_len - 1, a.kv_len - a.R + row0 + 8 * hr) - (key0 + c * 32) + 1;
+            vis[c] = nvis >= 32 ? 0xffffffffu : (nvis <= 0 ? 0u : ((1u << nvis) - 1u));
+          } else {
+            vis[c] = tc_vis_word(mrow[hr], words, key0 + c * 32 - prefix);
+          }
         }
-        tc_commit(&o_done[g]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[k_slot(0)], 0);
-      tc_fence_after();
-      issue_qk(0, 0);
-      issue_qk(1, 0);
-      tc_commit(&kv_empty[k_slot(0)]);
-      for (int j = 0; j < n_tiles; ++j) {
-        const bool more = j + 1 < n_tiles;
-        // group 0: its P is ready → its score accumulator is free: next scores first (group 0's softmax waits for them), then PV
-        mbar_wait(&p_full[0], (uint32_t)j & 1u);
-        if (more) {
-          mbar_wait(&kv_full[k_slot(j + 1)], (k_item(j + 1) / kTcSlots) & 1u);
-          tc_fence_after();
-          issue_qk(0, j + 1);
-        }
-        mbar_wait(&kv_full[v_slot(j)], (v_item(j) / kTcSlots) & 1u);
-        tc_fence_after();
-        issue_pv(0, j);
-        mbar_wait(&p_full[1], (uint32_t)j & 1u);
-        tc_fence_after();
-        if (more) {
-          issue_qk(1, j + 1);
-          tc_commit(&kv_empty[k_slot(j + 1)]);  // both score MMAs of tile j+1 have been issued: K slot free when they complete
-        }
-        issue_pv(1, j);
-        tc_commit(&kv_empty[v_slot(j)]);        // the V slot is consumed
+#pragma unroll
+        for (int n = 0; n < 16; ++n)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * n + 2 * t + e;
+            if (!((vis[col >> 5] >> (col & 31)) & 1u)) s[4 * n + 2 * hr + e] = -INFINITY;
+          }
       }
     }
-  } else if (warp >= 4) {
-    // ================= softmax warps: group g = query tile g; thread r <-> query row r <-> TMEM lane r =================
-    const int g = (warp - 4) >> 2;
-    const int wq = (warp - 4) & 3;              // TMEM lane quarter this warp may access (warp id % 4)
-    const int r = wq * 32 + lane;
-    const int row = qb * kTcBlockRows + g * kTcRows + r;
-    const uint32_t lane_base = (uint32_t)(wq * 32) << 16;
-    const uint32_t sacc = tmem + (uint32_t)g * 128u + lane_base;
-    const uint32_t oacc = tmem + 256u + (uint32_t)g * 128u + lane_base;
-    const int prefix = a.kv_len - a.tree_cols;
-    const int words = a.tree_cols >> 5;
-    const uint32_t* mrow = a.tree_mask != nullptr ? a.tree_mask + (size_t)min(row, a.R - 1) * words : nullptr;
-    float m_run = -INFINITY, l_run = 0.f;  // running maximum (log2 domain, already scaled) and denominator
-    const uint32_t p_row = smem_u32(p_s) + (uint32_t)g * kTcTileBytes + (uint32_t)r * 128u;
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(&s_full[g], (uint32_t)j & 1u);
-      tc_fence_after();
-      const int key0 = (t_begin + j) * kTcKeys;
-      // does this tile touch tree columns / the end of the keys / (causal) the diagonal of this block?  (uniform per CTA)
-      const bool masked_tile = a.causal ? key0 + kTcKeys - 1 > a.kv_len - a.R + qb * kTcBlockRows : key0 + kTcKeys > prefix;
-      if (a.debug_s != nullptr && j == 0 && qb == 0 && h == 0 && sp == 0 && g == 0) {  // test hook: the raw score tile
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t dbg[32];
-          tc_ld32(sacc + (uint32_t)c * 32u, dbg);
-          tc_wait_ld();
+    // ---- online softmax of the two rows (the four threads of a quad share a row) ----
+    float mref[2];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) a.debug_s[(size_t)r * 128 + c * 32 + i] = __uint_as_float(dbg[i]);
-        }
-      }
-      // ---- the whole score row into registers: four loads in flight, one wait ----
-      uint32_t v[4][32];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) tc_ld32(sacc + (uint32_t)c * 32u, v[c]);
-      tc_wait_ld();
-      if (masked_tile) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t vis;
-          if (a.causal) {  // keys key0+32c .. : visible up to lim = min(kv_len - 1, kv_len - R + row)
-            const int nvis = min(a.kv_len - 1, a.kv_len - a.R + row) - (key0 + c * 32) + 1;
-            vis = nvis >= 32 ? 0xffffffffu : (nvis <= 0 ? 0u : ((1u << nvis) - 1u));
-          } else {
-            vis = tc_vis_word(mrow, words, key0 + c * 32 - prefix);
-          }
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (!((vis >> i) & 1u)) v[c][i] = 0xff800000u;  // -inf
-        }
-      }
+    for (int hr = 0; hr < 2; ++hr) {
       float tmax = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 4; ++c)
+      for (int n = 0; n < 16; ++n) tmax = fmaxf(tmax, fmaxf(s[4 * n + 2 * hr], s[4 * n + 2 * hr + 1]));
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+      const float m_new = fmaxf(m_run[hr], tmax * a.scale_log2);  // -inf stays -inf
+      const float alpha = (m_run[hr] == -INFINITY) ? 0.f : tc_ex2(m_run[hr] - m_new);
+      l_run[hr] *= alpha;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) tmax = fmaxf(tmax, __uint_as_float(v[c][i]));
-      const float tm = tmax * a.scale_log2;  // -inf stays -inf
-      // lazy rescale: keep the old reference maximum unless the new one is more than 2^8 above it (p <= 256: exact enough in
-      // fp16 x fp32 accumulate); the decision is taken per warp because the TMEM accesses below are warp-collective
-      const bool grow = tm > m_run + kTcLazyLog2 || (m_run == -INFINITY && tm > -INFINITY);
-      const bool warp_grow = __any_sync(0xffffffffu, grow);
-      float m_new = m_run;
-      if (warp_grow) m_new = fmaxf(m_run, tm);
-      // P_g and O_g are free once the previous PV of this group has completed
-      if (j > 0) {
-        mbar_wait(&o_done[g], ((uint32_t)(j - 1)) & 1u);
-        tc_fence_after();
-        if (warp_grow) {
-          const float alpha = (m_run == -INFINITY) ? 0.f : tc_ex2(m_run - m_new);
-          l_run *= alpha;
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tc_ld32(oacc + (uint32_t)c * 32u, o);
-            tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tc_st32(oacc + (uint32_t)c * 32u, o);
-          }
-          tc_wait_st();
-        }
+      for (int n = 0; n < 16; ++n) {
+        o[4 * n + 2 * hr] *= alpha;
+        o[4 * n + 2 * hr + 1] *= alpha;
       }
-      m_run = m_new;
-      const float mref = (m_run == -INFINITY) ? 0.f : m_run;
-      // ---- p = exp2(s*scale - m), denominator, fp16 pack into the swizzled K-major P tile ----
-      float lsum = 0.f;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t packed[16];
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = tc_ex2(fmaf(__uint_as_float(v[c][i]), a.scale_log2, -mref));
-          const float p1 = tc_ex2(fmaf(__uint_as_float(v[c][i + 1]), a.scale_log2, -mref));
-          lsum += p0 + p1;
-          const __half2 hp = __floats2half2_rn(p0, p1);
-          packed[i >> 1] = *reinterpret_cast<const uint32_t*>(&hp);
-        }
-        // keys c*32 .. c*32+31 of this row = four 16-byte chunks; chunk index within the 64-key half = (c & 1) * 4 + q
-        const uint32_t half_off = (uint32_t)(c >> 1) * kTcHalfBytes;
-#pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          const uint32_t chunk = (uint32_t)(c & 1) * 4u + (uint32_t)q4;
-          const uint32_t addr = p_row + half_off + ((chunk ^ ((uint32_t)r & 7u)) << 4);
-          asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(packed[q4 * 4]), "r"(packed[q4 * 4 + 1]), "r"(packed[q4 * 4 + 2]),
-                       "r"(packed[q4 * 4 + 3])
-                       : "memory");
-        }
-      }
-      l_run += lsum;
-      tc_fence_before();              // the TMEM reads of S_g are complete: the MMA warp may overwrite it after p_full
-      fence_proxy_async();            // the generic-proxy stores of P must be visible to the tensor core (async proxy)
-      mbar_arrive(&p_full[g]);
+      m_run[hr] = m_new;
+      mref[hr] = (m_new == -INFINITY) ? 0.f : m_new;
     }
-    // ---- publish the partial of this (block, head, split) ----
-    const size_t slot = ((size_t)qb * a.H + h) * a.splits + sp;
-    const int rb = g * kTcRows + r;  // row within the 256-row block
-    float* po = a.part_o + (slot * kTcBlockRows + rb) * kTcD;
-    if (n_tiles > 0) {
-      mbar_wait(&o_done[g], ((uint32_t)(n_tiles - 1)) & 1u);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t o[32];
-        tc_ld32(oacc + (uint32_t)c * 32u, o);
-        tc_wait_ld();
+    // ---- p = exp2(s*scale - m), denominator, fp16 pack straight into the A fragments of PV ----
+    uint32_t pa[32];
 #pragma unroll
-        for (int i = 0; i < 32; i += 4)
-          *reinterpret_cast<float4*>(po + c * 32 + i) = make_float4(__uint_as_float(o[i]), __uint_as_float(o[i + 1]), __uint_as_float(o[i + 2]), __uint_as_float(o[i + 3]));
+    for (int n = 0; n < 16; ++n)
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const float p0 = tc_ex2(fmaf(s[4 * n + 2 * hr], a.scale_log2, -mref[hr]));
+        const float p1 = tc_ex2(fmaf(s[4 * n + 2 * hr + 1], a.scale_log2, -mref[hr]));
+        l_run[hr] += p0 + p1;
+        pa[4 * (n >> 1) + 2 * (n & 1) + hr] = pack_half2(p0, p1);
       }
-    }
-    a.part_m[slot * kTcBlockRows + rb] = n_tiles > 0 ? m_run : -INFINITY;
-    a.part_l[slot * kTcBlockRows + rb] = n_tiles > 0 ? l_run : 0.f;
+    // ---- O += P V ----
+    mbar_wait(&kv_full[vs], vph);
+    const uint32_t v_u = smem_u32(kv_s + (size_t)vs * kTcTileBytes);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < kTcKeys / 16; ++kk)  // B = V [128 keys][128 d] MN-major: 16 keys = 16 rows of 128 B; d halves 16 KB apart
+      wg_mma_rs_tb(o, &pa[4 * kk], wg_desc(v_u + (uint32_t)kk * 16u * 128u, kTcHalfBytes, 1024));
+    wg_commit();
+    wg_wait_all();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[vs]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc_dealloc(tmem, 512);
+  // ---- publish the partial of this (block, head, split) ----
+  const size_t slot = ((size_t)qb * a.H + h) * a.splits + sp;
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int rb = rb0 + 8 * hr;
+    float l = l_run[hr];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    if (n_tiles > 0) {
+      float* po = a.part_o + (slot * kTcBlockRows + rb) * kTcD;
+#pragma unroll
+      for (int n = 0; n < 16; ++n) *reinterpret_cast<float2*>(po + 8 * n + 2 * t) = make_float2(o[4 * n + 2 * hr], o[4 * n + 2 * hr + 1]);
+    }
+    if (t == 0) {
+      a.part_m[slot * kTcBlockRows + rb] = n_tiles > 0 ? m_run[hr] : -INFINITY;
+      a.part_l[slot * kTcBlockRows + rb] = n_tiles > 0 ? l : 0.f;
+    }
+  }
 }
 
 // out[row][h][:] = sum_s 2^(m_s - m) O_s / sum_s 2^(m_s - m) l_s over the KV splits (fixed order → deterministic)
@@ -447,7 +343,7 @@ typedef CUresult (*PFN_encodeTiledTC)(CUtensorMap*, CUtensorMapDataType, cuuint3
 
 static int tc_plan_splits(int blocks, int H, int tiles_total) {
   int sms = sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   // enough CTAs for >= ~8 waves of one-CTA-per-SM work items, but never fewer than 16 tiles per split
   int splits = (8 * sms + blocks * H - 1) / (blocks * H);
   const int max_splits = tiles_total / 16 > 0 ? tiles_total / 16 : 1;
@@ -500,7 +396,7 @@ int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensor
   {
     cuuint64_t gdim[3] = {(cuuint64_t)d, (cuuint64_t)H, (cuuint64_t)R};
     cuuint64_t gstride[2] = {(cuuint64_t)d * 2, (cuuint64_t)H * d * 2};
-    cuuint32_t box[3] = {64, 1, (cuuint32_t)kTcRows};
+    cuuint32_t box[3] = {64, 1, (cuuint32_t)kTcBlockRows};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = encode(&qmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(q), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -525,14 +421,8 @@ int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensor
   a.part_m = a.part_o + slots * kTcBlockRows * kTcD;
   a.part_l = a.part_m + slots * kTcBlockRows;
   a.debug_s = debug_scores;
-  const size_t smem = 1024 + (size_t)(4 + kTcSlots) * kTcTileBytes + 256;
-  int dev = 0;
-  TF_CHECK_CUDA(cudaGetDevice(&dev));
-  static bool attr_done[64] = {false};
-  if (dev >= 64 || !attr_done[dev]) {
-    TF_CHECK_CUDA(cudaFuncSetAttribute(tree_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (dev < 64) attr_done[dev] = true;
-  }
+  const size_t smem = 1024 + (size_t)(1 + kTcSlots) * kTcTileBytes + 256;
+  TF_ENSURE_DYNAMIC_SMEM(tree_attn_tc_kernel, smem);
   tree_attn_tc_kernel<<<dim3(blocks, H, splits), kTcThreads, smem, stream>>>(qmap, kmap, vmap, a);
   TF_CHECK_LAUNCH();
   tree_attn_merge_kernel<<<dim3(R, H), 128, 0, stream>>>(a.part_o, a.part_m, a.part_l, H, R, splits, (__half*)out);

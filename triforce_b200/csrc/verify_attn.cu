@@ -14,9 +14,9 @@
 //     keep the FP32 pipe out of the way, not because the problem is compute bound;
 //   * per-(CTA, head) partials (m, l, O) go to a small workspace; the LAST CTA to deliver a partial of a head (an
 //     arrival counter per head, self-resetting) merges that head's <= G/H + 2 partials — no second launch.
-//   * the split is equal by default.  Measured with %globaltimer stamps per CTA (tools/attn_timing.py): SMs of a B200 do
-//     not pull the same HBM bandwidth — under an equal split the same SMs finish their ranges at 228 us and others at
-//     294 us in every launch (GPC-level sharing), so the kernel waits ~13% on the slowest GPCs.  tf_verify_attn_calibrate
+//   * the split is equal by default.  SMs need not all pull the same HBM bandwidth (GPC-level sharing; per-CTA
+//     %globaltimer stamps show it, tools/attn_timing.py), so under an equal split the kernel waits on the slowest GPCs.
+//     tf_verify_attn_calibrate
 //     measures the per-CTA streaming time of this very kernel and stores a cumulative split table (fractions of the tile
 //     axis per blockIdx) in the workspace; launches with the same grid then cut the axis in proportion to the measured
 //     per-CTA rate.  The table only moves segment boundaries: per-(CTA, head) partials and their merge order stay a pure
@@ -554,7 +554,7 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
 
 static int g_max_slots() {
   int sms = sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   return sms * 2;
 }
 
@@ -577,8 +577,8 @@ static int launch_mma(const CUtensorMap& kmap, const CUtensorMap& vmap, const __
     if (dev < 64) attr_done[dev] = true;
   }
   // Programmatic launch only for short stores: the long (full-KV) launches use the calibrated per-CTA split, which assumes the
-  // block placement of a launch onto an EMPTY GPU — an early launch next to a draining predecessor changes it and costs more
-  // than the overlap gains (measured: profiles/r02_profile_step_pdl.md).  They still trigger their own dependents early.
+  // block placement of a launch onto an EMPTY GPU — an early launch next to a draining predecessor changes it, which
+  // can cost more than the overlap gains.  They still trigger their own dependents early.
   TF_CHECK_CUDA(launch_kernel(allow_pdl ? kPdlVerifyAttn : 0, kern, G, kThreadsAttn, smem, stream, kmap, vmap, q, layer, kv_len_host, kv_len_dev, R, H, scale_log2, pm, pl, po, counters,
                               out, tree_mask, tree_cols, split_table, cta_ns, clean_keys, pf_ptr, pf_chunks));
   TF_CHECK_LAUNCH();

@@ -1,4 +1,4 @@
-"""Llama target / draft forward passes around the sm_100a hot-path kernels.
+"""Llama target / draft forward passes around the sm_90a hot-path kernels.
 
 Restates the dataflow of the reference's `models/modeling_llama.py:200-414` (target, YaRN RoPE, full / retrieval cache
 routing) and `models/modeling_llama_68m.py:129-357` (Llama-68M draft, StreamingLLM cache, RoPE re-applied at slot
@@ -7,7 +7,7 @@ q/k/v/gate/up, row-split o/down, one all-reduce after each).  Decode-time projec
 the SiLU·mul epilogue, down_proj, lm_head with the fp32 epilogue) run on this repo's weight-streaming kernel
 (`tf_stream_linear`, SURVEY §8 row f-1), so a decode / verify forward launches nothing but this library's kernels and chains
 them with programmatic dependent launch; prefill-sized GEMMs (> 24 rows) stay on cuBLAS through `F.linear` (plain library GEMMs).
-The long-prompt PREFILL attention (q_len > 32) runs on this repo's tcgen05 kernel in causal mode for head_dim 128
+The long-prompt PREFILL attention (q_len > 32) runs on this repo's wgmma kernel in causal mode for head_dim 128
 (`tf_tree_attn_tc`, SURVEY §8 row f-2); the 64-wide heads of the parity-sized models keep the library call (flash-attn / SDPA).
 """
 from __future__ import annotations
@@ -131,7 +131,7 @@ class LlamaModel:
         self.peer_stream = None     # the same on tf_stream_linear (exchange of tile t hidden behind the weights of tile t+1)
         self.prefill_tc = os.environ.get("TRIFORCE_PREFILL_TC", "1") == "1" and self.device.type == "cuda"
         # retrieval-verify attention prefetching the o_proj weights into L2 while it is latency-bound (tf_verify_attn_prefetch).
-        # OPT-IN: measured on cfg2 it LOSES (retrieval verify 3.43 -> 3.51 ms, profiles/r02_attn_l2_prefetch_ab.json): the requests
+        # OPT-IN (not measured faster on H100): the requests
         # compete with the K/V tiles of the attention they ride on, and o_proj's own ring fill under PDL already covers its start.
         self.attn_prefetch = os.environ.get("TRIFORCE_ATTN_PREFETCH", "0") == "1" and self.use_stream_linear
         self._tc_ws, self._tc_ws_key = None, None
@@ -162,7 +162,7 @@ class LlamaModel:
         self.m_lm_head = mk(self.lm_head)
 
     def _tc_workspace(self, rows: int, maps) -> torch.Tensor:
-        """Split-partial workspace of the tcgen05 attention (tf_tree_attn_tc) for `rows` query rows over this store."""
+        """Split-partial workspace of the wgmma attention (tf_tree_attn_tc) for `rows` query rows over this store."""
         key = (rows, self.local_num_heads, int(maps.shape[2]))
         if self._tc_ws_key != key:
             self._tc_ws = None  # release the old one first
@@ -177,9 +177,11 @@ class LlamaModel:
     def calibrate_attention(self, kv_cache, rows: int = 7, rounds: int = 4) -> Optional[dict]:
         """Init-time load balancing of the verify attention on this GPU (tf_verify_attn_calibrate): the kernel's per-CTA key
         ranges are re-cut in proportion to the HBM rate each CTA actually gets.  `rows` <= 16 calibrates the grid of the
-        decode / verify launches, 17..32 the one-CTA-per-SM grid of the 32-row tree blocks.  TRIFORCE_ATTN_CALIBRATE=0 keeps
-        the equal split.  Short stores (< 16K keys) are left alone — there is nothing to balance."""
-        if os.environ.get("TRIFORCE_ATTN_CALIBRATE", "1") != "1" or self.is_draft:
+        decode / verify launches, 17..32 the one-CTA-per-SM grid of the 32-row tree blocks.  OPT-IN (TRIFORCE_ATTN_CALIBRATE=1):
+        on an H100 the equal split is faster (full-KV verify at 124 944 keys: 0.684 ms equal vs 0.721-0.726 ms calibrated per
+        layer) and, unlike a split measured at start-up, bit-reproducible across processes.  Short stores (< 16K keys) are left
+        alone — there is nothing to balance."""
+        if os.environ.get("TRIFORCE_ATTN_CALIBRATE", "0") != "1" or self.is_draft:
             return None
         maps = kv_cache.tensor_maps
         cap = int(maps.shape[2])
@@ -203,7 +205,7 @@ class LlamaModel:
         """NVLink seam exchange for decode-sized messages (PeerAllReduce: LL slots pushed through NVLS multicast stores, by default
         straight from the seam projection's epilogue and summed inside the following add+RMSNorm).  `max_rows` = largest message
         in rows of `hidden` (0 = automatic: 24 rows = every tf_stream_linear launch, so cfg4's gamma+1 = 17-row verifies stay on
-        it; 8 rows for the round-1 pull kernel, which lost to NCCL from 17 rows up — profiles/r01_allreduce_check_tp2.log).
+        it; 8 rows for the round-1 pull kernel, which is meant for small messages).
         Larger messages (prefill) go through NCCL.  The older fused GEMV + all-reduce kernels stay opt-in
         (TRIFORCE_FUSED_LINEAR_ALLREDUCE=1, TRIFORCE_STREAM_ALLREDUCE=1)."""
         if max_rows <= 0:
@@ -213,9 +215,9 @@ class LlamaModel:
             self.peer_allreduce = PeerAllReduce(self.device, self.tp_rank, self.tp_world, max_rows * self.config.hidden_size * 2)
             if os.environ.get("TRIFORCE_FUSED_LINEAR_ALLREDUCE", "0") == "1":
                 self.peer_linear = PeerFusedLinear(self.device, self.tp_rank, self.tp_world)
-            # the seams as one kernel each: tf_stream_linear with the all-reduce in its epilogue.  OPT-IN: measured at 2 GPUs
-            # (profiles/r02_tp2*.json) the seam projections have ~1 tile per CTA (N = 4096, K long), so the exchange of a tile
-            # has no next tile to hide behind and the separate PDL-chained one-shot kernel is faster (26.99 vs 29.18 ms/step).
+            # the seams as one kernel each: tf_stream_linear with the all-reduce in its epilogue.  OPT-IN: the seam projections
+            # have ~1 tile per CTA (N = 4096, K long), so the exchange of a tile has no next tile to hide behind, and the
+            # separate PDL-chained one-shot kernel is expected to be faster (not measured on H100).
             if self.use_stream_linear and os.environ.get("TRIFORCE_STREAM_ALLREDUCE", "0") == "1":
                 self.peer_stream = PeerStreamLinear(self.device, self.tp_rank, self.tp_world)
 
@@ -333,7 +335,7 @@ class LlamaModel:
                                 variant=self.attn_variant)
                 return out
             if d == 128 and self.prefill_tc:
-                # prompt chunks on the tcgen05 kernel in causal mode (SURVEY §8 row f-2): no library call on the 7B / 13B path
+                # prompt chunks on the wgmma kernel in causal mode (SURVEY §8 row f-2): no library call on the 7B / 13B path
                 ops.tree_attn_tc(q_out, kv_cache.tensor_maps, l, old_len + n, n, Hl, d, self.scale, None, 0, out,
                                  self._tc_workspace(n, kv_cache.tensor_maps), causal=True)
                 return out
@@ -362,7 +364,7 @@ class LlamaModel:
         Hl, d = self.local_num_heads, self.head_dim
         n = q_out.shape[0]
         if d == 128 and n >= 128 and n % 128 == 0 and os.environ.get("TRIFORCE_TREE_TC", "1") == "1":
-            # the whole tree in ONE pass over the KV on the tcgen05 tensor cores (variant 2; reads each KV byte n/128 times
+            # the whole tree in ONE pass over the KV on the tensor cores (wgmma, variant 2; reads each KV byte n/128 times
             # instead of n/32 times)
             ops.tree_attn_tc(q_out, maps, layer, kv_len, n, Hl, d, self.scale, mask_bits, tree_cols, out, self._tc_workspace(n, maps))
             return

@@ -157,7 +157,7 @@ def tree_attn_tc_workspace(R: int, H: int, kv_len_max: int, device) -> torch.Ten
 
 def tree_attn_tc(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, H: int, d: int, scale: float, tree_mask: Optional[torch.Tensor],
                  tree_cols: int, out, workspace, debug_scores: Optional[torch.Tensor] = None, causal: bool = False):
-    """tcgen05 / TMEM attention (tf_tree_attn_tc), d = 128: tree-verify (`tree_mask` as in verify_attn_tree), plain, or — with
+    """wgmma tensor-core attention (tf_tree_attn_tc), d = 128: tree-verify (`tree_mask` as in verify_attn_tree), plain, or — with
     causal=True — the bottom-right causal attention of R new rows over kv_len keys (prefill chunks)."""
     require_cuda(q, out, workspace)
     _f16c(q, "q")

@@ -6,7 +6,7 @@ The target model with its RETRIEVAL cache grows a static 512-node token tree in 
 KV verifies it; the accepted root-to-leaf path is walked with recursive rejection sampling and the accepted nodes' KV rows
 are compacted into the cache (`gather_kv_incremental`).
 
-B200 mapping: both masked attentions run on `tf_verify_attn_tree` (prefix fully visible + a 512-bit ancestor mask per
+GPU mapping: both masked attentions run on `tf_verify_attn_tree` (prefix fully visible + a 512-bit ancestor mask per
 row, 32 query rows per launch); the accept walk (SpecTree.accept_step :147-165 + verify :181-197) is ONE kernel
 (`tf_tree_accept_walk`) instead of ~5 host round-trips per examined child; top-p + softmax of the 512 target rows is
 `tf_norm_logits`; the KV compaction is `tf_kv_compact`.  The reference's 5 broadcast+barrier pairs per verify (:205-223)

@@ -6,8 +6,8 @@ One process per GPU (`torchrun`), NCCL over NVLink/NVSwitch for the two all-redu
 attention — full KV, retrieval cache, per-head top-k selection, draft — is rank-local (SURVEY §8e).  The reference's
 rank-0-samples-then-broadcast (+barrier) protocol (decoding.py:230-239,350-351) is replaced by identically seeded
 replicated sampling: the logits are bit-identical on every rank after the all-reduce, so every rank draws the same token
-with no communication.  KV offloading (`kv_offload`, `on_chip_layers`) is accepted and ignored: a B200 holds the whole
-128K KV in HBM (SURVEY §2a marks the offload path out of scope).
+with no communication.  KV offloading (`kv_offload`, `on_chip_layers`) is accepted and ignored: the whole KV stays in
+HBM — split over the ranks' GPUs — (SURVEY §2a marks the offload path out of scope).
 """
 from __future__ import annotations
 
