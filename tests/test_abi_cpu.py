@@ -55,6 +55,21 @@ def test_unsupported_shapes_are_rejected():
     assert lib.tf_verify_attn(p, p, p, 0, 64, None, 64, 4, 1, 96, 0.1, p, p, 1 << 30, 0, 0, None) == -2   # head_dim 96
     assert lib.tf_norm_logits(p, 70000, 1, 70000, 1.0, 0.9, p, None, 0, None) == -2                    # vocab too large
     assert lib.tf_verify_attn_workspace_bytes(8, 32, 128) > 0
+    # tf_tree_attn_tc(q, kmap, vmap, layer, kv_len, R, H, d, scale, tree_mask, tree_cols, causal, out, ws, ws_bytes, dbg, stream)
+    a = (p + 15) & ~15  # 16-byte aligned workspace
+    R, H, S = 512, 32, 4096
+    ws = lib.tf_tree_attn_tc_workspace_bytes(R, H, S)
+    assert ws > 0
+    assert lib.tf_tree_attn_tc(p, p, p, 0, S, R, H, 64, 0.1, p, 512, 0, p, a, ws, None, None) == -2   # head_dim 64
+    assert lib.tf_tree_attn_tc(p, p, p, 0, S, R, H, 128, 0.1, p, 512, 1, p, a, ws, None, None) == -1  # causal with a tree
+    assert b"causal" in lib.tf_last_error()
+    assert lib.tf_tree_attn_tc(p, p, p, 0, S, R, H, 128, 0.1, p, 500, 0, p, a, ws, None, None) == -1  # tree_cols % 32
+    assert b"multiple of 32" in lib.tf_last_error()
+    assert lib.tf_tree_attn_tc(p, p, p, 0, S, R, H, 128, 0.1, p, 512, 0, p, a, ws - 1, None, None) == -1  # workspace 1 B short
+    assert b"workspace" in lib.tf_last_error()
+    # the exact workspace size passes that check: the call stops at the next one (a misaligned q), before any launch
+    assert lib.tf_tree_attn_tc(a + 2, p, p, 0, S, R, H, 128, 0.1, p, 512, 0, p, a, ws, None, None) == -1
+    assert b"q must be 16-byte aligned" in lib.tf_last_error()
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):

@@ -638,7 +638,7 @@ def test_stream_linear_under_programmatic_dependent_launch():
         torch.cuda.synchronize()
         assert torch.equal(out, want)
     finally:
-        lib.tf_set_pdl(int(os.environ.get("TRIFORCE_PDL", "0")))
+        lib.tf_set_pdl(int(os.environ.get("TRIFORCE_PDL", str(_C.DEFAULT_PDL_MASK))))  # the mask _C.lib() loaded with
 
 
 @pytest.mark.parametrize("M,inter,K", [(1, 11008, 4096), (7, 11008, 4096), (8, 13824, 5120), (16, 5504, 4096), (8, 24, 64), (5, 1376, 4096),
