@@ -11,6 +11,7 @@ Files written:
   retrieval_build.npz   reference RetrievalCache.init_graph_cache: fp16 chunk scores, raw torch.topk indices, cache rows
   sampling.npz          reference norm_logits / max_fn on seeded logits
   forward.npz           reference target forward: last-token logits after a chunked prefill, retrieval-verify logits
+  yarn_7b_rows.npz      rows of the reference's YaRN cos/sin tables at the 7B / 13B geometry (see yarn_7b_row_indices)
   e2e_<cfg>.json        event traces (every sample / rand / Middle_Spec return / target input) of TriForce first and
                         second call (the draft-cache reset quirk, SURVEY §7 hard part 3) and of Autoregressive
   ref_*                 the reference's PG-19 loader, tree file and command lines (see make_reference_files)
@@ -151,6 +152,28 @@ def make_forward():
                         yarn_cos_rows=rot.cos_cached[:: 97].numpy(), yarn_sin_rows=rot.sin_cached[:: 97].numpy())
     assert np.array_equal(logits_last.astype(np.float16).astype(np.float32), logits_last)
     print("[forward] wrote logits; |logits| max", np.abs(logits_last).max())
+
+
+YARN_7B_STRIDE = 1021  # strided rows over the whole 131 072-row table
+
+
+def yarn_7b_row_indices(max_pos: int = 131072) -> np.ndarray:
+    """Rows of yarn_7b_rows.npz: every 1021st row, every row of 124 900..124 999 (around the cfg2 prompt end, where fp32
+    positions times inv_freq are furthest from exact) and the last 64 rows."""
+    rows = np.concatenate([np.arange(0, max_pos, YARN_7B_STRIDE), np.arange(124900, 125000), np.arange(max_pos - 64, max_pos)])
+    return np.unique(rows).astype(np.int64)
+
+
+def make_yarn_7b():
+    """The reference's LlamaYaRNRotaryEmbedding at the 7B / 13B geometry (head_dim 128, 131 072 positions, factor 32 over an
+    original 4096), built on the CPU as the reference builds it (modeling_llama.py:187-194)."""
+    ref = rh.load_reference()
+    rot = ref.ml.LlamaYaRNRotaryEmbedding(128, max_position_embeddings=131072, base=10000, scaling_factor=32.0,
+                                          original_max_position_embeddings=4096)
+    rows = yarn_7b_row_indices()
+    np.savez_compressed(os.path.join(HERE, "yarn_7b_rows.npz"), rows=rows, cos=rot.cos_cached[rows].numpy(),
+                        sin=rot.sin_cached[rows].numpy())
+    print(f"[yarn_7b] wrote {len(rows)} rows of the 131072 x 128 tables")
 
 
 def make_e2e():
@@ -303,7 +326,7 @@ def make_reference_files():
 
 
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["retrieval", "sampling", "forward", "e2e", "tree", "reference_files"]
+    which = sys.argv[1:] or ["retrieval", "sampling", "forward", "yarn_7b", "e2e", "tree", "reference_files"]
     with torch.inference_mode():
         if "retrieval" in which:
             make_retrieval_build()
@@ -311,6 +334,8 @@ if __name__ == "__main__":
             make_sampling()
         if "forward" in which:
             make_forward()
+        if "yarn_7b" in which:
+            make_yarn_7b()
         if "e2e" in which:
             make_e2e()
         if "tree" in which:

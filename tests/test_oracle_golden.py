@@ -76,6 +76,22 @@ def test_rope_tables_match_reference_rows(golden_dir):
     assert np.abs(ocos[::97].astype(np.float32) - g["yarn_cos_rows"].astype(np.float32)).max() <= 2e-3
 
 
+def test_rope_tables_match_reference_rows_7b_geometry(golden_dir):
+    """The 7B / 13B YaRN tables (head_dim 128, 131 072 positions, factor 32 over 4096): strided rows over the whole table,
+    every row of 124 900..124 999 and the last 64 rows must equal the reference's bit for bit.  Near position 125K the
+    fp32 product t * inv_freq is off by several fp16 ulps of cos / sin from the exact angle, so only the reference's own
+    recipe reproduces these rows."""
+    from triforce_b200.rope import tables_for
+    g = np.load(os.path.join(golden_dir, "yarn_7b_rows.npz"))
+    rows = g["rows"]
+    assert set(range(124900, 125000)) <= set(rows.tolist()) and rows.max() == 131071 and len(rows) > 200
+    cos, sin = tables_for(named_config("llama-7B-128K"))
+    assert tuple(cos.shape) == (131072, 128)
+    np.testing.assert_array_equal(cos[rows].numpy(), g["cos"])
+    np.testing.assert_array_equal(sin[rows].numpy(), g["sin"])
+    assert tables_for(named_config("llama-13B-128K"))[0].shape == cos.shape  # same head_dim, positions and scaling
+
+
 def assert_logits_close(actual, desired, what=""):
     """BASELINE north_star tolerance for verify logits is rtol 1e-2 / atol 1e-3 (fp16).  Logits are fp16 numbers of
     magnitude ~1-3 (ulp 1e-3..2e-3), produced by two different fp16 pipelines, so a sliver of elements sits one or two
