@@ -9,14 +9,14 @@ wrongly admits then moves the output far outside the tolerance.  Rows past kv_le
 the softmax if they were read.  Each test also checks that its comparison rejects mutated references (a KV split dropped,
 the causal diagonal shifted, a tree-mask bit flipped, one key too many), so the tolerance is known to see those errors;
 the negative controls launch no library kernel."""
-import math
 import os
-import time
 
 import numpy as np
 import pytest
 import torch
 
+from attn_needles import (STALE_V, Needles, assert_rejected, base_logit, excess, plant_stale, reference,
+                          report_time_and_memory, visibility)  # noqa: F401  (report_time_and_memory: autouse fixture)
 from oracle import triforce_oracle as orc
 from triforce_b200 import _C, ops
 from triforce_b200.spectree import load_grow_map
@@ -27,81 +27,11 @@ D = 128             # head dim (tf_tree_attn_tc supports only 128)
 TILE = 128          # keys per tile of tf_tree_attn_tc
 BLOCK_ROWS = 128    # query rows per CTA of tf_tree_attn_tc
 SCALE = orc.softmax_scale_fp16(D)
-Q_ALONG = 8.0       # component of every query row along its head's shared direction
-NEEDLE_V = 4.0      # |V| of a needle row (random signs)
-STALE_V = 16.0      # |V| of a stale row past kv_len
-
-
-@pytest.fixture(autouse=True)
-def _report_time_and_memory(request):
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    yield
-    torch.cuda.synchronize()
-    print(f"\n[{request.node.name}] {time.perf_counter() - t0:.1f} s, peak device memory "
-          f"{torch.cuda.max_memory_allocated() / 2**30:.2f} GiB")
-    torch.cuda.empty_cache()
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# fp64 reference, tolerance, split plan
+# split plan
 # ---------------------------------------------------------------------------------------------------------------------
-def visibility(R: int, n_keys: int, kv_len: int, causal: bool = False, tree: torch.Tensor = None) -> torch.Tensor:
-    """bool [R, n_keys]: does query row i see key j?
-    causal: row i sees key j iff j <= kv_len - R + i (the R rows are the last R keys);
-    tree:   the first kv_len - T keys are seen by every row, key kv_len - T + c by the rows whose tree[i, c] is set;
-    no row sees a key >= kv_len."""
-    i = torch.arange(R, device=DEV)[:, None]
-    j = torch.arange(n_keys, device=DEV)[None, :]
-    if causal:
-        vis = j <= kv_len - R + i
-    else:
-        T = 0 if tree is None else tree.shape[1]
-        vis = (j < kv_len - T).expand(R, n_keys).clone()
-        if T:
-            vis[:, kv_len - T:kv_len] = tree
-    return vis & (j < kv_len)
-
-
-def reference(q: torch.Tensor, K: torch.Tensor, V: torch.Tensor, vis: torch.Tensor) -> torch.Tensor:
-    """One head in fp64: q [R, D], K / V [>= n, D] (fp16 store rows), vis [R, n] → softmax(scale · q Kᵀ, masked by vis) · V;
-    a row that sees no key gets zeros (as the kernels write)."""
-    n = vis.shape[1]
-    s = (q.double() @ K[:n].double().T) * SCALE
-    s.masked_fill_(~vis, float("-inf"))
-    return torch.softmax(s, dim=-1).nan_to_num_(0.0) @ V[:n].double()
-
-
-# Error budget of a kernel output against the fp64 reference, relative to the head's output scale:
-#   * output rounded to fp16 ............................ <= 2^-11 |want| (half an ulp)
-#   * P rounded to fp16 before the P·V wgmma (the softmax denominator sums the unrounded fp32 P)
-#                                                     ... <= 2^-11 sum_j p_j |v_j| / l per element, about 2^-11 of the
-#                                                         head's output scale here: the needles carry most of the mass
-#                                                         and the needle at the row maximum has P = 1 exactly
-#   * ex2.approx.ftz (2 ulp of fp32), fp32 scores of exact fp16 products, the fp32 split merge ... below 2^-20
-# Sum: about 2^-10 of the output scale.  The tolerance allows twice that: rtol 2^-9 and atol 2^-9 of the head's largest
-# output, and never more than assert_attn_close's (rtol 1e-2, atol 2e-3).
-RTOL = 2.0 ** -9
-ATOL_CAP = 2e-3
-
-
-def excess(got: torch.Tensor, want: torch.Tensor) -> float:
-    """max |got - want| / (atol + RTOL |want|) over one head's [R, D] outputs, atol = min(ATOL_CAP, RTOL max|want|):
-    <= 1 passes."""
-    atol = min(ATOL_CAP, RTOL * want.abs().max().item())
-    err = (got.double() - want).abs().nan_to_num(nan=float("inf"))
-    return (err / (atol + RTOL * want.abs())).max().item()
-
-
-def assert_rejected(mutants, want: torch.Tensor, what: str):
-    """Negative controls: each (name, mutant reference) must fail the comparison against the real reference."""
-    for name, m in mutants:
-        e = excess(m, want)
-        assert e > 1.0, f"{what}: the comparison does not reject the mutant '{name}' (excess {e:.3g})"
-
-
 def cdiv(a: int, b: int) -> int:
     return -(-a // b)
 
@@ -136,45 +66,8 @@ def split_key_ranges(R: int, kv_len: int, splits: int, causal: bool):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# inputs with needles
+# tree needles and the per-head comparison
 # ---------------------------------------------------------------------------------------------------------------------
-def base_logit(kv_len: int) -> float:
-    """Needle logit (scale · q·k): background scores have a standard deviation of about SCALE·sqrt(Q_ALONG² + D) ≈ 1.2, so
-    the background weighs about kv_len·e^0.75; a needle at ln(kv_len) + 3 outweighs all of it ~10 times."""
-    return math.log(kv_len) + 3.0
-
-
-class Needles:
-    """Per-head unit directions u_h; query rows Q_ALONG·u_h plus noise orthogonal to u_h; needle keys b·u_h with
-    q·k = Q_ALONG·b set to a chosen logit; needle V rows ±NEEDLE_V with random signs."""
-
-    def __init__(self, H: int, seed: int):
-        self.H = H
-        self.g = torch.Generator(device=DEV).manual_seed(seed)
-        u = torch.randn((H, D), generator=self.g, device=DEV, dtype=torch.float64)
-        self.u = u / u.norm(dim=-1, keepdim=True)
-
-    def store(self, L: int, cap: int) -> torch.Tensor:
-        return torch.randn((L, self.H, cap, D), generator=self.g, device=DEV, dtype=torch.float16)
-
-    def queries(self, R: int) -> torch.Tensor:
-        n = torch.randn((R, self.H, D), generator=self.g, device=DEV, dtype=torch.float64)
-        n -= (n * self.u).sum(-1, keepdim=True) * self.u
-        return (Q_ALONG * self.u + n).half().contiguous()
-
-    def plant(self, K, V, layer: int, keys, logits, v_amp: float = NEEDLE_V):
-        keys = torch.as_tensor(list(keys), device=DEV, dtype=torch.long)
-        b = torch.as_tensor(list(logits), device=DEV, dtype=torch.float64) / (SCALE * Q_ALONG)
-        K[layer, :, keys] = (b[None, :, None] * self.u[:, None, :]).half()
-        signs = torch.randint(0, 2, (self.H, keys.numel(), D), generator=self.g, device=DEV).double() * 2 - 1
-        V[layer, :, keys] = (v_amp * signs).half()
-
-
-def plant_stale(nd: Needles, K, V, layer: int, kv_len: int, cap: int):
-    """Rows kv_len .. cap-1 (left over from a longer sequence, e.g. after kv_compact): keys far above every needle."""
-    nd.plant(K, V, layer, range(kv_len, cap), [base_logit(kv_len) + 8.0] * (cap - kv_len), v_amp=STALE_V)
-
-
 def tree_needle_column(tree: torch.Tensor):
     """A tree column seen by some rows and not by others, and a row that does not see it."""
     seen = tree.sum(0)
