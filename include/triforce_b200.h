@@ -69,6 +69,16 @@ int tf_retrieval_build(const void* K, const void* V, long long kv_layer_stride, 
                        const void* q, int n_layers, int H, int d, int prefill, int chunk, int budget,
                        void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride,
                        int32_t* out_idx, void* out_scores, void* workspace, size_t workspace_bytes, tf_stream_t stream);
+/* tf_retrieval_build_gqa: the build of a grouped-query-attention target (Hq query heads over Hkv KV heads, query head h reads
+ *   KV head h / (Hq/Hkv)) under the "group_sum" rule.  The reference defines no GQA rule (cache.py:157 broadcasts q over KV
+ *   heads); this one scores each (layer, KV head) with q̄ = the sum of its group's query heads, taken in fp64 (exact for up to
+ *   64 heads per group):  score = fp16(q̄·k̄) with the dot as above, then top-k and gather per (layer, KV head) exactly as above.
+ *   Hkv == Hq gives tf_retrieval_build's bits.  q fp16 [n_layers][Hq][d]; out_idx [n_layers][Hkv][budget/chunk];
+ *   out_scores [n_layers][Hkv][prefill/chunk]; the workspace is tf_retrieval_build_workspace_bytes(n_layers, Hkv, ...). */
+int tf_retrieval_build_gqa(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride,
+                           const void* q, int n_layers, int Hq, int Hkv, int d, int prefill, int chunk, int budget,
+                           void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride,
+                           int32_t* out_idx, void* out_scores, void* workspace, size_t workspace_bytes, tf_stream_t stream);
 
 /* ---- fused RoPE + KV append --------------------------------------------------------------------------------------
  * replaces models/modeling_llama.py:217-230 (apply_rotary_pos_emb + FlashSimpleCache.update cache.py:52-53 /
@@ -86,6 +96,13 @@ int tf_rope_append(const void* q, const void* k, const void* v, long long qkv_ro
                    const void* sin, int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev,
                    int slot0, const int32_t* slot0_dev, int R, int H, int d, int rotate_q, int rotate_k, void* q_out,
                    void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream);
+/* tf_rope_append_gqa: the same for Hq query heads and Hkv K/V heads (Hq % Hkv == 0): q [R][Hq*d] → q_out [R][Hq][d], k / v
+ *   [R][Hkv*d] (row stride qkv_row_stride, e.g. slices of one [Hq·d | Hkv·d | Hkv·d] GEMM row) appended to Hkv cache heads.
+ *   Hkv == Hq gives tf_rope_append's bits. */
+int tf_rope_append_gqa(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos,
+                       const void* sin, int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev,
+                       int slot0, const int32_t* slot0_dev, int R, int Hq, int Hkv, int d, int rotate_q, int rotate_k,
+                       void* q_out, void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream);
 
 /* ---- (iii) verify attention over the retrieval budget or the full KV ------------------------------------------
  * replaces flash_attn_with_kvcache at models/modeling_llama.py:240 (and tensor_op.py:166-168,316): causal,
@@ -119,6 +136,24 @@ int tf_verify_attn_prefetch(const void* q, const void* k_tensormap, const void* 
                             size_t workspace_bytes, int variant, int clean_keys, const void* next_weights, size_t next_weight_bytes,
                             tf_stream_t stream);
 
+/* tf_verify_attn_gqa: tf_verify_attn for grouped-query attention — Hq query heads over a store of Hkv KV heads, Hq % Hkv == 0,
+ *   query head h reads KV head h / G (G = Hq / Hkv, Hugging Face `repeat_kv` order).  q / out fp16 [R][Hq][d].  The stream-K
+ *   units are (KV head, key tile); one CTA computes the R·G rows of a whole group against each tile it loads, so every K/V byte
+ *   is read once per launch (kv_len·Hkv·d·2·2 bytes).  Packed row i = token row i / G of query head kvh·G + i % G; the causal
+ *   limit and the tree-mask row are those of the token row.  R·G <= TF_VERIFY_MAX_ROWS (larger requests are cut into blocks
+ *   of token rows by the caller, each with the kv_len that keeps it bottom-right aligned).  Workspace:
+ *   tf_verify_attn_gqa_workspace_bytes (partials and arrival counters per KV head), zero-filled before first use.  G = 1 runs
+ *   the code and gives the bits of tf_verify_attn.  There is no calibrated split or L2 prefetch for these launches.
+ * tf_verify_attn_tree_gqa: the same for tf_verify_attn_tree; tree_mask is [R][tree_cols/32] over TOKEN rows. */
+size_t tf_verify_attn_gqa_workspace_bytes(int R, int Hq, int Hkv, int d);
+int tf_verify_attn_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
+                       const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv, int d, float scale, void* out,
+                       void* workspace, size_t workspace_bytes, int variant, int clean_keys, tf_stream_t stream);
+int tf_verify_attn_tree_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
+                            const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv, int d, float scale,
+                            const uint32_t* tree_mask, int tree_cols, void* out, void* workspace, size_t workspace_bytes,
+                            tf_stream_t stream);
+
 /* tf_tree_attn_tc: the tree (Sequoia) verify attention on the Hopper tensor cores — `variant 2` of the verify attention, for
  *   R = 128·k query rows (the 512 tree nodes of BASELINE cfg5) against the full KV of one layer; replaces the SDPA call with an
  *   additive [512, S+512] mask at models/tensor_op.py:230-272 / utils/SpecTree_TP.py:168-175.  One CTA = (128-row block, head, KV
@@ -134,6 +169,12 @@ size_t tf_tree_attn_tc_workspace_bytes(int R, int H, int kv_len_max);
 int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int H, int d,
                     float scale, const uint32_t* tree_mask, int tree_cols, int causal, void* out, void* workspace,
                     size_t workspace_bytes, float* debug_scores, tf_stream_t stream);
+/* tf_tree_attn_tc_gqa: tf_tree_attn_tc for Hq query heads over Hkv KV heads (query head h reads KV head h / (Hq/Hkv)).  The grid,
+ *   the workspace (tf_tree_attn_tc_workspace_bytes(R, Hq, kv_len_max)), q, out and the merge stay per query head; the CTAs of
+ *   one group read the same K/V tiles, through L2 (the kernel is tensor-bound). */
+int tf_tree_attn_tc_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int Hq,
+                        int Hkv, int d, float scale, const uint32_t* tree_mask, int tree_cols, int causal, void* out,
+                        void* workspace, size_t workspace_bytes, tf_stream_t stream);
 
 /* Init-time load balancing of tf_verify_attn (no reference counterpart; the reference has no such knob).  The kernel cuts
  * its (head, key-tile) axis into one contiguous range per CTA.  Where the SMs of a GPU do not all pull the same HBM bandwidth,

@@ -28,6 +28,19 @@ _SIGNATURES = {
     "tf_retrieval_build": (c_int, [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                    c_int, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,
                                    c_size_t, c_void_p]),
+    "tf_retrieval_build_gqa": (c_int, [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                       c_int, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,
+                                       c_size_t, c_void_p]),
+    "tf_rope_append_gqa": (c_int, [c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                   c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                   c_void_p, c_longlong, c_longlong, c_void_p]),
+    "tf_verify_attn_gqa_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "tf_verify_attn_gqa": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                   c_float, c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
+    "tf_verify_attn_tree_gqa": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                        c_float, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tf_tree_attn_tc_gqa": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int,
+                                    c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "tf_rope_append": (c_int, [c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                c_longlong, c_longlong, c_void_p]),

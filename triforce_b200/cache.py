@@ -139,8 +139,9 @@ class RetrievalCache(_HeadMajorStore):
     def init_graph_cache(self, kv_cache: FlashSimpleCache, query_states: torch.Tensor, layer_idx: int):
         """Per-layer build (cache.py:146-178).  query_states: [1, 1, H, d] post-RoPE query of the last prompt token."""
         assert 1 == query_states.shape[1], "query_states should be 1 for init"
-        q = query_states.reshape(1, self.num_heads, self.head_dim).contiguous()
-        ops.retrieval_build(kv_cache.key_store, kv_cache.value_store, q, self.key_store, self.value_store, self.prefill,
+        q = query_states.reshape(1, -1, self.head_dim).contiguous()
+        build = ops.retrieval_build if q.shape[1] == self.num_heads else ops.retrieval_build_gqa  # GQA: the "group_sum" rule
+        build(kv_cache.key_store, kv_cache.value_store, q, self.key_store, self.value_store, self.prefill,
                             self.chunk_size, self.max_budget, layer0=layer_idx, n_layers=1,
                             out_idx=self.topk_idx[layer_idx:layer_idx + 1], out_scores=self.chunk_scores[layer_idx:layer_idx + 1])
         if layer_idx == self.layers - 1:
@@ -148,8 +149,10 @@ class RetrievalCache(_HeadMajorStore):
 
     def build_all_layers(self, kv_cache: FlashSimpleCache, queries: torch.Tensor):
         """All layers in ONE launch sequence (3 kernels instead of 3*L): `queries` [L, H, d].  The selection of layer l
-        only needs that layer's query and full K, both final once the last prompt token has gone through layer l."""
-        ops.retrieval_build(kv_cache.key_store, kv_cache.value_store, queries.contiguous(), self.key_store, self.value_store,
+        only needs that layer's query and full K, both final once the last prompt token has gone through layer l.
+        A grouped-query target passes its Hq query heads and is scored by the "group_sum" rule (tf_retrieval_build_gqa)."""
+        build = ops.retrieval_build if queries.shape[1] == self.num_heads else ops.retrieval_build_gqa
+        build(kv_cache.key_store, kv_cache.value_store, queries.contiguous(), self.key_store, self.value_store,
                             self.prefill, self.chunk_size, self.max_budget, layer0=0, n_layers=self.layers,
                             out_idx=self.topk_idx, out_scores=self.chunk_scores)
         self.init_graph = True

@@ -27,13 +27,27 @@ class LlamaShape:
     rope_scaling: Optional[dict] = None
     initializer_range: float = 0.02
     name: str = "llama"
+    # How a grouped-query target (num_key_value_heads < num_attention_heads) scores retrieval chunks.  The reference defines
+    # no rule (cache.py:157 broadcasts q over kv heads), so a GQA shape must name one.  "group_sum": each KV head scores a
+    # chunk with the fp64 sum of its group's query heads (tf_retrieval_build_gqa).  Ignored for MHA shapes.
+    gqa_retrieval: Optional[str] = None
+
+    GQA_RETRIEVAL_RULES = ("group_sum",)
 
     def __post_init__(self):
         if self.num_key_value_heads is None:
             self.num_key_value_heads = self.num_attention_heads
-        # The reference's retrieval scoring broadcasts q heads against kv heads (cache.py:157): MHA only.
         if self.num_key_value_heads != self.num_attention_heads:
-            raise ValueError("TriForce hot path is MHA-only (reference models/cache.py:157 broadcasts q over kv heads)")
+            if self.gqa_retrieval is None:
+                # The reference's retrieval scoring broadcasts q heads against kv heads (cache.py:157): MHA only, unless the
+                # shape names a GQA retrieval rule.
+                raise ValueError("TriForce hot path is MHA-only (reference models/cache.py:157 broadcasts q over kv heads); "
+                                 f"a grouped-query shape must name a gqa_retrieval rule {self.GQA_RETRIEVAL_RULES}")
+            if self.gqa_retrieval not in self.GQA_RETRIEVAL_RULES:
+                raise ValueError(f"unknown gqa_retrieval rule {self.gqa_retrieval!r}; known: {self.GQA_RETRIEVAL_RULES}")
+            if self.num_key_value_heads < 1 or self.num_attention_heads % self.num_key_value_heads:
+                raise ValueError(f"num_attention_heads ({self.num_attention_heads}) must be a multiple of "
+                                 f"num_key_value_heads ({self.num_key_value_heads})")
         if self.hidden_size % self.num_attention_heads:
             raise ValueError("hidden_size must be divisible by num_attention_heads")
 
@@ -48,7 +62,8 @@ class LlamaShape:
 
     def param_count(self) -> int:
         h, i, L, v = self.hidden_size, self.intermediate_size, self.num_hidden_layers, self.vocab_size
-        return 2 * v * h + L * (4 * h * h + 3 * h * i + 2 * h) + h
+        hkv = self.num_key_value_heads * self.head_dim  # k_proj / v_proj rows
+        return 2 * v * h + L * (2 * h * h + 2 * hkv * h + 3 * h * i + 2 * h) + h
 
     def kv_bytes_per_token_layer(self) -> int:
         return 2 * self.num_key_value_heads * self.head_dim * 2  # K+V, fp16
@@ -61,6 +76,10 @@ def named_config(name: str) -> LlamaShape:
         # NousResearch/Yarn-Llama-2-7b-128k
         "llama-7B-128K": dict(hidden_size=4096, intermediate_size=11008, num_hidden_layers=32, num_attention_heads=32,
                               max_position_embeddings=131072, rope_scaling=yarn32, rms_norm_eps=1e-5),
+        # synthetic grouped-query geometry (no checkpoint): llama-7B-128K with 8 KV heads and a 14336-wide MLP
+        "llama-7B-gqa8-128K": dict(hidden_size=4096, intermediate_size=14336, num_hidden_layers=32, num_attention_heads=32,
+                                   num_key_value_heads=8, max_position_embeddings=131072, rope_scaling=yarn32, rms_norm_eps=1e-5,
+                                   gqa_retrieval="group_sum"),
         # NousResearch/Yarn-Llama-2-13b-128k
         "llama-13B-128K": dict(hidden_size=5120, intermediate_size=13824, num_hidden_layers=40, num_attention_heads=40,
                                max_position_embeddings=131072, rope_scaling=yarn32, rms_norm_eps=1e-5),

@@ -20,12 +20,13 @@ __global__ void __launch_bounds__(D / 4) rope_append_kernel(const __half* __rest
                                                             const __half* __restrict__ cos, const __half* __restrict__ sin,
                                                             int max_pos, const int32_t* __restrict__ pos_ids, int pos0,
                                                             const int32_t* __restrict__ pos0_dev, int slot0,
-                                                            const int32_t* __restrict__ slot0_dev, int H, int rotate_q,
+                                                            const int32_t* __restrict__ slot0_dev, int H, int Hkv, int rotate_q,
                                                             int rotate_k, __half* __restrict__ q_out,
                                                             __half* __restrict__ Kc, __half* __restrict__ Vc,
                                                             long long head_stride, long long cap) {
   pdl_launch_dependents();
   pdl_wait();
+  // one CTA per (row, query head); the first Hkv of them also append K/V head h (grouped-query attention: Hkv < H)
   const int r = blockIdx.x, h = blockIdx.y, j = threadIdx.x;  // j-th half2 of the first half
   int pos = pos_ids ? pos_ids[r] : pos0 + (pos0_dev ? *pos0_dev : 0) + r;
   pos = min(max(pos, 0), max_pos - 1);
@@ -42,7 +43,7 @@ __global__ void __launch_bounds__(D / 4) rope_append_kernel(const __half* __rest
     o[j] = lo;
     o[j + D / 4] = hi;
   }
-  if (slot >= 0 && slot < cap) {
+  if (h < Hkv && slot >= 0 && slot < cap) {
     const size_t dst = (size_t)h * head_stride + (size_t)slot * D;
     const __half2* x = reinterpret_cast<const __half2*>(k + in);
     __half2 lo = x[j], hi = x[j + D / 4];
@@ -312,13 +313,15 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const __half* __restrict_
 
 extern "C" {
 
-int tf_rope_append(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
-                   int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
-                   const int32_t* slot0_dev, int R, int H, int d, int rotate_q, int rotate_k, void* q_out, void* Kcache,
-                   void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream_) {
+// H query heads, Hkv K/V heads (Hkv == H: MHA)
+static int rope_append_impl(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
+                            int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
+                            const int32_t* slot0_dev, int R, int H, int Hkv, int d, int rotate_q, int rotate_k, void* q_out,
+                            void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream_) {
   using namespace tf;
   TF_CHECK_ARG(q && k && v && cos && sin && q_out && Kcache && Vcache, "tf_rope_append: NULL pointer");
   TF_CHECK_ARG(R >= 1 && H >= 1 && max_pos >= 1 && cap >= 1, "tf_rope_append: bad extents");
+  TF_CHECK_ARG(Hkv >= 1 && H % Hkv == 0, "tf_rope_append_gqa: Hq (%d) must be a positive multiple of Hkv (%d)", H, Hkv);
   TF_CHECK_SUPPORTED(d == 64 || d == 128, "tf_rope_append: head_dim %d not in {64,128}", d);
   TF_CHECK_ARG(qkv_row_stride % 2 == 0 && kv_head_stride % 2 == 0, "tf_rope_append: strides must be even");
   if (!slot0_dev) TF_CHECK_ARG(slot0 >= 0 && (long long)slot0 + R <= cap, "tf_rope_append: slots [%d,%d) exceed capacity %lld", slot0, slot0 + R, cap);
@@ -327,15 +330,31 @@ int tf_rope_append(const void* q, const void* k, const void* v, long long qkv_ro
   if (d == 128)
     TF_CHECK_CUDA(launch_kernel(kPdlRope, rope_append_kernel<128>, grid, 32, 0, stream, (const __half*)q, (const __half*)k, (const __half*)v, qkv_row_stride,
                                                      (const __half*)cos, (const __half*)sin, max_pos, pos_ids_dev, pos0, pos0_dev,
-                                                     slot0, slot0_dev, H, rotate_q, rotate_k, (__half*)q_out, (__half*)Kcache,
+                                                     slot0, slot0_dev, H, Hkv, rotate_q, rotate_k, (__half*)q_out, (__half*)Kcache,
                                                      (__half*)Vcache, kv_head_stride, cap));
   else
     TF_CHECK_CUDA(launch_kernel(kPdlRope, rope_append_kernel<64>, grid, 16, 0, stream, (const __half*)q, (const __half*)k, (const __half*)v, qkv_row_stride,
                                                     (const __half*)cos, (const __half*)sin, max_pos, pos_ids_dev, pos0, pos0_dev,
-                                                    slot0, slot0_dev, H, rotate_q, rotate_k, (__half*)q_out, (__half*)Kcache,
+                                                    slot0, slot0_dev, H, Hkv, rotate_q, rotate_k, (__half*)q_out, (__half*)Kcache,
                                                     (__half*)Vcache, kv_head_stride, cap));
   TF_CHECK_LAUNCH();
   return TF_OK;
+}
+
+int tf_rope_append(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
+                   int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
+                   const int32_t* slot0_dev, int R, int H, int d, int rotate_q, int rotate_k, void* q_out, void* Kcache,
+                   void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream) {
+  return rope_append_impl(q, k, v, qkv_row_stride, cos, sin, max_pos, pos_ids_dev, pos0, pos0_dev, slot0, slot0_dev, R, H, H, d,
+                          rotate_q, rotate_k, q_out, Kcache, Vcache, kv_head_stride, cap, stream);
+}
+
+int tf_rope_append_gqa(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
+                       int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
+                       const int32_t* slot0_dev, int R, int Hq, int Hkv, int d, int rotate_q, int rotate_k, void* q_out,
+                       void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream) {
+  return rope_append_impl(q, k, v, qkv_row_stride, cos, sin, max_pos, pos_ids_dev, pos0, pos0_dev, slot0, slot0_dev, R, Hq, Hkv, d,
+                          rotate_q, rotate_k, q_out, Kcache, Vcache, kv_head_stride, cap, stream);
 }
 
 int tf_draft_attn(const void* q, const void* K, const void* V, long long kv_head_stride, const void* cos, const void* sin,

@@ -4,6 +4,8 @@
 //   k̄[c]   = fp16( fp32 sum over the chunk's rows in row order * fp32(1/chunk) )
 //   score  = fp16( fp64 dot: slices of 8 consecutive d elements summed in order, slice partials butterfly-combined )
 //   order  = descending score, ascending chunk index on ties, -0 == +0, NaN greatest; chunk 0 forced first.
+// Grouped-query attention (tf_retrieval_build_gqa, rule "group_sum"): scores, top-k and gather run per (layer, KV head) and
+// the score's query is q̄ = fp64 sum of the grp query heads of the group (exact for grp <= 64 fp16 values); grp = 1 is MHA.
 // All three kernels are HBM/latency bound integer+fp work; no tensor cores (task statement ①).
 #include "common.cuh"
 
@@ -16,7 +18,7 @@ namespace tf {
 template <int D, int CHUNK /* 0 = runtime */>
 __global__ void __launch_bounds__(256) chunk_score_kernel(const __half* __restrict__ K, long long layer_stride,
                                                           long long head_stride, const __half* __restrict__ q,
-                                                          int H, int chunks, int chunk_rt, __half* __restrict__ scores) {
+                                                          int H, int qg, int chunks, int chunk_rt, __half* __restrict__ scores) {
   constexpr int LPR = D / 8;        // lanes per row
   constexpr int CPW = 32 / LPR;     // chunks per warp pass
   const int chunk = CHUNK ? CHUNK : chunk_rt;
@@ -24,13 +26,15 @@ __global__ void __launch_bounds__(256) chunk_score_kernel(const __half* __restri
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int grp = lane / LPR, li = lane % LPR;
   const __half* Kh = K + (size_t)layer * layer_stride + (size_t)h * head_stride;
-  const __half* qh = q + ((size_t)layer * H + h) * D + li * 8;
+  const __half* qh = q + ((size_t)layer * H + h) * qg * D + li * 8;  // the qg query heads of KV head h
   double q64[8];
-  {
-    uint4 raw = *reinterpret_cast<const uint4*>(qh);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) q64[i] = 0.0;
+  for (int g = 0; g < qg; ++g) {
+    uint4 raw = *reinterpret_cast<const uint4*>(qh + (size_t)g * D);
     const __half* qq = reinterpret_cast<const __half*>(&raw);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) q64[i] = (double)__half2float(qq[i]);
+    for (int i = 0; i < 8; ++i) q64[i] += (double)__half2float(qq[i]);
   }
   const float inv = 1.0f / (float)chunk;
   const int warps_per_grid = gridDim.x * (blockDim.x >> 5);
@@ -74,7 +78,7 @@ __global__ void __launch_bounds__(256) chunk_score_kernel(const __half* __restri
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const float mean16 = __half2float(__float2half_rn(__fmul_rn(acc[i], inv)));
-      part = fma((double)mean16, q64[i], part);  // product exact in fp64 → same as mul+add
+      part = __dadd_rn(part, __dmul_rn((double)mean16, q64[i]));  // not fused: a group sum q̄ may carry more than 42 bits
     }
 #pragma unroll
     for (int m = LPR / 2; m >= 1; m >>= 1) part += __shfl_xor_sync(0xffffffffu, part, m);
@@ -202,6 +206,12 @@ static int next_pow2(int x) {
 
 extern "C" {
 
+// H = KV heads of the store; the query has H * grp heads (grp = 1: MHA)
+static int retrieval_build_impl(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
+                                int n_layers, int H, int grp, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
+                                long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
+                                void* workspace, size_t workspace_bytes, tf_stream_t stream_);
+
 size_t tf_retrieval_build_workspace_bytes(int n_layers, int H, int d, int prefill, int chunk, int budget) {
   if (n_layers <= 0 || H <= 0 || chunk <= 0) return 0;
   const size_t chunks = (size_t)(prefill / chunk), sel = (size_t)(budget / chunk);
@@ -212,7 +222,27 @@ size_t tf_retrieval_build_workspace_bytes(int n_layers, int H, int d, int prefil
 int tf_retrieval_build(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
                        int n_layers, int H, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
                        long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
-                       void* workspace, size_t workspace_bytes, tf_stream_t stream_) {
+                       void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  return retrieval_build_impl(K, V, kv_layer_stride, kv_head_stride, q, n_layers, H, 1, d, prefill, chunk, budget, retrK, retrV,
+                              r_layer_stride, r_head_stride, out_idx, out_scores, workspace, workspace_bytes, stream);
+}
+
+int tf_retrieval_build_gqa(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
+                           int n_layers, int Hq, int Hkv, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
+                           long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
+                           void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0 || Hq / Hkv > 64) {
+    tf::set_error("tf_retrieval_build_gqa: Hq (%d) must be a multiple of Hkv (%d), at most 64 per KV head", Hq, Hkv);
+    return TF_ERR_INVALID;
+  }
+  return retrieval_build_impl(K, V, kv_layer_stride, kv_head_stride, q, n_layers, Hkv, Hq / Hkv, d, prefill, chunk, budget, retrK,
+                              retrV, r_layer_stride, r_head_stride, out_idx, out_scores, workspace, workspace_bytes, stream);
+}
+
+static int retrieval_build_impl(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
+                                int n_layers, int H, int grp, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
+                                long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
+                                void* workspace, size_t workspace_bytes, tf_stream_t stream_) {
   using namespace tf;
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(K && V && q && retrK && retrV, "tf_retrieval_build: NULL pointer");
@@ -253,7 +283,7 @@ int tf_retrieval_build(const void* K, const void* V, long long kv_layer_stride, 
     dim3 grid(gx, H, n_layers);
 #define LAUNCH_SCORE(D_, C_)                                                                                        \
   chunk_score_kernel<D_, C_><<<grid, 256, 0, stream>>>((const __half*)K, kv_layer_stride, kv_head_stride,          \
-                                                       (const __half*)q, H, chunks, chunk, scores)
+                                                       (const __half*)q, H, grp, chunks, chunk, scores)
     if (d == 128) { if (chunk == 8) LAUNCH_SCORE(128, 8); else LAUNCH_SCORE(128, 0); }
     else if (d == 64) { if (chunk == 8) LAUNCH_SCORE(64, 8); else LAUNCH_SCORE(64, 0); }
     else { if (chunk == 8) LAUNCH_SCORE(256, 8); else LAUNCH_SCORE(256, 0); }

@@ -21,6 +21,11 @@
 //              32 KB tiles in the order K0 V0 K1 V1 ...; a slot is released when both warpgroups' wgmmas that read it completed.
 //   The two warpgroups are independent: while one runs its softmax, the tensor core serves the other's wgmmas.
 // Partials (m, l, unnormalised O) per (block, head, split) go to the workspace; `tree_attn_merge_kernel` combines the splits.
+//
+// Grouped-query attention (tf_tree_attn_tc_gqa): the grid stays (block, QUERY head, split) and only the producer's K/V head
+// coordinate becomes h / grp.  The grp CTAs of a group each stream the same K/V tiles, so KV is read grp times per block
+// instead of once.  That is acceptable here: this kernel is bound by the tensor cores (2·128 FLOP per byte), the group's
+// CTAs run side by side, and the repeated reads hit L2.
 #include <string.h>
 
 #include "common.cuh"
@@ -91,6 +96,7 @@ __device__ __forceinline__ void tc_tma_3d(uint32_t smem_dst, const CUtensorMap* 
 
 struct TcArgs {
   int layer, H, R;
+  int grp;                    // query heads per KV head: query head h reads K/V head h / grp (1: MHA)
   int kv_len;                 // keys (prefix + tree columns)
   int tree_cols;              // last tree_cols keys follow the bitmask (0: every key below kv_len is visible to every row)
   const uint32_t* tree_mask;  // [R][tree_cols / 32]
@@ -184,7 +190,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
         for (int half = 0; half < 2; ++half) {
 #pragma unroll
           for (int kb = 0; kb < 2; ++kb)  // the KV tensor maps carry 64-key boxes: two per 128-key tile, stacked row after row
-            tma_load_4d(dst + half * kTcHalfBytes + kb * (kTcHalfBytes / 2), map, &kv_full[s], half * 64, key0 + kb * 64, h, a.layer);
+            tma_load_4d(dst + half * kTcHalfBytes + kb * (kTcHalfBytes / 2), map, &kv_full[s], half * 64, key0 + kb * 64, h / a.grp, a.layer);
         }
       }
     }
@@ -365,10 +371,10 @@ size_t tf_tree_attn_tc_workspace_bytes(int R, int H, int kv_len_max) {
   return slots * kTcBlockRows * (kTcD + 2) * sizeof(float) + 256;
 }
 
-// q fp16 [R][H][128] contiguous; out fp16 [R][H][128].  debug_scores: nullable, fp32 [128][128].
-int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int H, int d, float scale,
-                    const uint32_t* tree_mask, int tree_cols, int causal, void* out, void* workspace, size_t workspace_bytes,
-                    float* debug_scores, tf_stream_t stream_) {
+// q fp16 [R][H][128] contiguous; out fp16 [R][H][128]; H query heads over H / grp KV heads.  debug_scores: nullable, fp32 [128][128].
+static int tree_attn_tc_impl(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int H,
+                             int grp, int d, float scale, const uint32_t* tree_mask, int tree_cols, int causal, void* out,
+                             void* workspace, size_t workspace_bytes, float* debug_scores, tf_stream_t stream_) {
   using namespace tf;
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(q && k_tensormap && v_tensormap && out && workspace, "tf_tree_attn_tc: NULL pointer");
@@ -411,7 +417,7 @@ int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensor
   const int tiles_total = (kv_len + kTcKeys - 1) / kTcKeys;
   const int splits = tc_plan_splits(blocks, H, tiles_total);
   TcArgs a;
-  a.layer = layer; a.H = H; a.R = R; a.kv_len = kv_len; a.tree_cols = tree_cols; a.tree_mask = tree_cols > 0 ? tree_mask : nullptr;
+  a.layer = layer; a.H = H; a.R = R; a.grp = grp; a.kv_len = kv_len; a.tree_cols = tree_cols; a.tree_mask = tree_cols > 0 ? tree_mask : nullptr;
   a.causal = causal;
   a.scale_log2 = scale * 1.4426950408889634f;
   a.splits = splits;
@@ -428,6 +434,24 @@ int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensor
   tree_attn_merge_kernel<<<dim3(R, H), 128, 0, stream>>>(a.part_o, a.part_m, a.part_l, H, R, splits, (__half*)out);
   TF_CHECK_LAUNCH();
   return TF_OK;
+}
+
+int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int H, int d, float scale,
+                    const uint32_t* tree_mask, int tree_cols, int causal, void* out, void* workspace, size_t workspace_bytes,
+                    float* debug_scores, tf_stream_t stream) {
+  return tree_attn_tc_impl(q, k_tensormap, v_tensormap, layer, kv_len, R, H, 1, d, scale, tree_mask, tree_cols, causal, out, workspace,
+                           workspace_bytes, debug_scores, stream);
+}
+
+int tf_tree_attn_tc_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int Hq, int Hkv,
+                        int d, float scale, const uint32_t* tree_mask, int tree_cols, int causal, void* out, void* workspace,
+                        size_t workspace_bytes, tf_stream_t stream) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0) {
+    tf::set_error("tf_tree_attn_tc_gqa: Hq (%d) must be a positive multiple of Hkv (%d)", Hq, Hkv);
+    return TF_ERR_INVALID;
+  }
+  return tree_attn_tc_impl(q, k_tensormap, v_tensormap, layer, kv_len, R, Hq, Hq / Hkv, d, scale, tree_mask, tree_cols, causal, out,
+                           workspace, workspace_bytes, nullptr, stream);
 }
 
 }  // extern "C"

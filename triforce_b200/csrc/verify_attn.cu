@@ -13,7 +13,11 @@
 //     O += P V.  The contraction is only 2*R FLOP per KV byte, far below the tensor roofline — tensor cores are used to
 //     keep the FP32 pipe out of the way, not because the problem is compute bound;
 //   * per-(CTA, head) partials (m, l, O) go to a small workspace; the LAST CTA to deliver a partial of a head (an
-//     arrival counter per head, self-resetting) merges that head's <= G/H + 2 partials — no second launch.
+//     arrival counter per head, self-resetting) merges that head's <= G/H + 2 partials — no second launch;
+//   * grouped-query attention (tf_verify_attn_gqa: Hq query heads over Hkv KV heads, group size grp = Hq / Hkv, query
+//     head h reads KV head h / grp): the work units are (KV head, tile) and a CTA computes the R * grp packed rows of
+//     all query heads of a group against every tile it loads, so each K/V byte is still read once per launch.
+//     "Head" below means KV head; MHA is grp = 1 and runs the same code.
 //   * the split is equal by default.  SMs need not all pull the same HBM bandwidth (GPC-level sharing; per-CTA
 //     %globaltimer stamps show it, tools/attn_timing.py), so under an equal split the kernel waits on the slowest GPCs.
 //     tf_verify_attn_calibrate
@@ -107,7 +111,7 @@ constexpr int kPfChunk = 4096;  // bytes per L2 prefetch request (tf_verify_attn
 template <int D, int MT, int STAGES>
 __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_mma_kernel(
     const __grid_constant__ CUtensorMap kmap, const __grid_constant__ CUtensorMap vmap, const __half* __restrict__ q,
-    int layer, int kv_len_host, const int32_t* __restrict__ kv_len_dev, int R, int H, float scale_log2,
+    int layer, int kv_len_host, const int32_t* __restrict__ kv_len_dev, int R, int H, int grp, float scale_log2,
     float* __restrict__ part_m, float* __restrict__ part_l, float* __restrict__ part_o, int* __restrict__ head_counters,
     __half* __restrict__ out, const uint32_t* __restrict__ tree_mask, int tree_cols,
     const uint32_t* __restrict__ split_table, uint32_t* __restrict__ cta_ns, int clean_keys, const uint8_t* __restrict__ pf_ptr,
@@ -231,7 +235,10 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
   if (early) pdl_wait();  // q (and the fresh K/V rows the last tiles carry) come from the predecessor
   const int g = lane >> 2, tq = lane & 3;
   const int mtile = warp % MT, kslice = warp / MT;
-  const int row0 = mtile * 16 + g, row1 = row0 + 8;  // query rows owned by this thread
+  const int row0 = mtile * 16 + g, row1 = row0 + 8;  // packed query rows owned by this thread
+  // Packed row i is token row i / grp of query head h * grp + i % grp (grp = 1: MHA, packed row = token row).
+  const int rows = R * grp, Hq = H * grp;
+  const int tr0 = row0 / grp, tr1 = row1 / grp;
   const int kbase = kslice * KW;
 
   uint32_t it = 0;
@@ -244,15 +251,15 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
     // ---- Q fragments of this head (A operand, rows >= R are zero) ----
     uint32_t qa[DK][4];
     {
-      const __half* q0 = q + ((size_t)row0 * H + h) * D;
-      const __half* q1 = q + ((size_t)row1 * H + h) * D;
+      const __half* q0 = q + ((size_t)tr0 * Hq + h * grp + row0 % grp) * D;
+      const __half* q1 = q + ((size_t)tr1 * Hq + h * grp + row1 % grp) * D;
 #pragma unroll
       for (int kk = 0; kk < DK; ++kk) {
         const int c = kk * 16 + 2 * tq;
-        qa[kk][0] = row0 < R ? *reinterpret_cast<const uint32_t*>(q0 + c) : 0u;
-        qa[kk][1] = row1 < R ? *reinterpret_cast<const uint32_t*>(q1 + c) : 0u;
-        qa[kk][2] = row0 < R ? *reinterpret_cast<const uint32_t*>(q0 + c + 8) : 0u;
-        qa[kk][3] = row1 < R ? *reinterpret_cast<const uint32_t*>(q1 + c + 8) : 0u;
+        qa[kk][0] = row0 < rows ? *reinterpret_cast<const uint32_t*>(q0 + c) : 0u;
+        qa[kk][1] = row1 < rows ? *reinterpret_cast<const uint32_t*>(q1 + c) : 0u;
+        qa[kk][2] = row0 < rows ? *reinterpret_cast<const uint32_t*>(q0 + c + 8) : 0u;
+        qa[kk][3] = row1 < rows ? *reinterpret_cast<const uint32_t*>(q1 + c + 8) : 0u;
       }
     }
     // ---- which CTAs deliver partials of head h: the owners of its first and last tile ----
@@ -298,12 +305,13 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
         }
       }
 
-      // ---- mask.  Causal (bottom-right): row i sees key j iff j <= kv_len - R + i.  Tree (Sequoia) mode: the first
-      //      kv_len - T keys are visible to every row, the last T columns follow the row's bitmask (ancestors of the node) ----
+      // ---- mask.  Causal (bottom-right): token row r sees key j iff j <= kv_len - R + r.  Tree (Sequoia) mode: the first
+      //      kv_len - T keys are visible to every row, the last T columns follow the token row's bitmask (ancestors of the
+      //      node).  Both take the TOKEN row of a packed row, never the packed row. ----
       const int key_tile0 = (int)t * BN + kbase;
       if (tree_mask == nullptr) {
         if (key_tile0 + KW - 1 > kv_len - R) {
-          const int lim0 = kv_len - R + row0, lim1 = kv_len - R + row1;
+          const int lim0 = kv_len - R + tr0, lim1 = kv_len - R + tr1;
 #pragma unroll
           for (int n = 0; n < NB; ++n) {
             const int j = key_tile0 + n * 8 + 2 * tq;
@@ -317,8 +325,8 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
         const int prefix = kv_len - tree_cols;
         if (key_tile0 + KW - 1 >= prefix) {
           const int words = tree_cols >> 5;
-          const uint32_t* m0p = tree_mask + (size_t)min(row0, R - 1) * words;
-          const uint32_t* m1p = tree_mask + (size_t)min(row1, R - 1) * words;
+          const uint32_t* m0p = tree_mask + (size_t)min(tr0, R - 1) * words;
+          const uint32_t* m1p = tree_mask + (size_t)min(tr1, R - 1) * words;
 #pragma unroll
           for (int n = 0; n < NB; ++n) {
 #pragma unroll
@@ -440,8 +448,8 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       }
     }
     const size_t slot = (size_t)b + (size_t)h;
-    for (int i = threadIdx.x; i < R * D; i += kConsumerWarps * 32) part_o[slot * (size_t)(TF_VERIFY_MAX_ROWS * D) + i] = Osh[i];
-    for (int r = threadIdx.x; r < R; r += kConsumerWarps * 32) {
+    for (int i = threadIdx.x; i < rows * D; i += kConsumerWarps * 32) part_o[slot * (size_t)(TF_VERIFY_MAX_ROWS * D) + i] = Osh[i];
+    for (int r = threadIdx.x; r < rows; r += kConsumerWarps * 32) {
       float mc = -INFINITY;
       for (int w = 0; w < NKW; ++w) mc = fmaxf(mc, msh[w * 16 * MT + r]);
       const float mcu = (mc == -INFINITY) ? 0.f : mc * scale_log2;
@@ -477,7 +485,7 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       // thread's output slots is idle (rows 8..15), so it runs a SECOND independent partial stream there: twice the loads in flight,
       // half the dependent L2 round trips; the two streams are merged at the end.  Only for P > 16, i.e. never on unsharded or
       // parity-sized launches, whose merge order stays exactly as it was.
-      const bool dual = (KF == 4) && (MT == 1) && (R <= 8) && (P > 16);
+      const bool dual = (KF == 4) && (MT == 1) && (rows <= 8) && (P > 16);
       const int pstep = dual ? 2 * PB : PB;
       float4 acc[KF];
       float mr[KF], den[KF];
@@ -494,7 +502,7 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
             const int pidx = p0 + pp + (dual ? (k >> 1) * PB : 0);
             const int f = threadIdx.x + kk * (kConsumerWarps * 32);
             const int r = f / F4R;
-            const bool ok = (pidx < P) && (r < R);
+            const bool ok = (pidx < P) && (r < rows);
             const size_t sl = (size_t)b_first + (size_t)(ok ? pidx : 0) + (size_t)h;
             v[pp][k] = ok ? __ldcg(reinterpret_cast<const float4*>(part_o + sl * (size_t)(TF_VERIFY_MAX_ROWS * D)) + f) : make_float4(0.f, 0.f, 0.f, 0.f);
             pm_[pp][k] = ok ? __ldcg(&part_m[sl * TF_VERIFY_MAX_ROWS + r]) : -INFINITY;
@@ -537,12 +545,12 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
         if (dual && k >= KF / 2) continue;
         const int f = threadIdx.x + k * (kConsumerWarps * 32);
         const int r = f / F4R, c4 = f % F4R;
-        if (r < R) {
+        if (r < rows) {
           const float inv = 1.f / den[k];
           uint2 pk;
           pk.x = pack_half2(acc[k].x * inv, acc[k].y * inv);
           pk.y = pack_half2(acc[k].z * inv, acc[k].w * inv);
-          *reinterpret_cast<uint2*>(out + ((size_t)r * H + h) * D + c4 * 4) = pk;
+          *reinterpret_cast<uint2*>(out + ((size_t)(r / grp) * Hq + h * grp + r % grp) * D + c4 * 4) = pk;
         }
       }
     }
@@ -560,7 +568,7 @@ static int g_max_slots() {
 
 template <int D, int MT, int STAGES>
 static int launch_mma(const CUtensorMap& kmap, const CUtensorMap& vmap, const __half* q, int layer, int kv_len_host,
-                      const int32_t* kv_len_dev, int R, int H, float scale_log2, float* pm, float* pl, float* po, int* counters,
+                      const int32_t* kv_len_dev, int R, int H, int grp, float scale_log2, float* pm, float* pl, float* po, int* counters,
                       __half* out, int G, const uint32_t* tree_mask, int tree_cols, const uint32_t* split_table, uint32_t* cta_ns,
                       int clean_keys, bool allow_pdl, cudaStream_t stream, const uint8_t* pf_ptr, uint32_t pf_chunks) {
   auto kern = verify_attn_mma_kernel<D, MT, STAGES>;
@@ -579,7 +587,7 @@ static int launch_mma(const CUtensorMap& kmap, const CUtensorMap& vmap, const __
   // Programmatic launch only for short stores: the long (full-KV) launches use the calibrated per-CTA split, which assumes the
   // block placement of a launch onto an EMPTY GPU — an early launch next to a draining predecessor changes it, which
   // can cost more than the overlap gains.  They still trigger their own dependents early.
-  TF_CHECK_CUDA(launch_kernel(allow_pdl ? kPdlVerifyAttn : 0, kern, G, kThreadsAttn, smem, stream, kmap, vmap, q, layer, kv_len_host, kv_len_dev, R, H, scale_log2, pm, pl, po, counters,
+  TF_CHECK_CUDA(launch_kernel(allow_pdl ? kPdlVerifyAttn : 0, kern, G, kThreadsAttn, smem, stream, kmap, vmap, q, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, pm, pl, po, counters,
                               out, tree_mask, tree_cols, split_table, cta_ns, clean_keys, pf_ptr, pf_chunks));
   TF_CHECK_LAUNCH();
   return TF_OK;
@@ -630,6 +638,12 @@ size_t tf_verify_attn_workspace_bytes(int R, int H, int d) {
   return attn_workspace((void*)0, H, d).bytes + 256;  // + worst-case alignment of the caller's base pointer
 }
 
+// partials, counters and split tables are per KV head: the MHA workspace of Hkv heads
+size_t tf_verify_attn_gqa_workspace_bytes(int R, int Hq, int Hkv, int d) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0) return 0;
+  return tf_verify_attn_workspace_bytes(R, Hkv, d);
+}
+
 struct AttnPlan {
   int G;          // grid
   int table_idx;  // which split table this grid uses
@@ -653,8 +667,9 @@ static AttnPlan attn_plan(int R, int H, int d, int kv_len_max) {
   return p;
 }
 
+// H = KV heads, grp = query heads per KV head (1: MHA); q / out are [R][H * grp][d]
 static int verify_attn_impl(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
-                            const int32_t* kv_len_dev, int kv_len_max, int R, int H, int d, float scale, void* out,
+                            const int32_t* kv_len_dev, int kv_len_max, int R, int H, int grp, int d, float scale, void* out,
                             void* workspace, size_t workspace_bytes, int variant, const uint32_t* tree_mask, int tree_cols,
                             bool record_cta_ns, int clean_keys, tf_stream_t stream_, const void* next_weights = nullptr,
                             size_t next_weight_bytes = 0) {
@@ -662,6 +677,8 @@ static int verify_attn_impl(const void* q, const void* k_tensormap, const void* 
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(q && k_tensormap && v_tensormap && out && workspace, "tf_verify_attn: NULL pointer");
   TF_CHECK_ARG(R >= 1 && R <= TF_VERIFY_MAX_ROWS, "tf_verify_attn: R=%d outside [1,%d]", R, TF_VERIFY_MAX_ROWS);
+  TF_CHECK_ARG(grp >= 1 && R * grp <= TF_VERIFY_MAX_ROWS,
+               "tf_verify_attn_gqa: R=%d rows x %d query heads per KV head exceed %d packed rows", R, grp, TF_VERIFY_MAX_ROWS);
   TF_CHECK_SUPPORTED(d == 64 || d == 128, "tf_verify_attn: head_dim %d not in {64,128}", d);
   TF_CHECK_ARG(H >= 1 && layer >= 0, "tf_verify_attn: bad H/layer");
   TF_CHECK_ARG(kv_len_dev || kv_len_host >= R, "tf_verify_attn: kv_len (%d) must include the %d new rows", kv_len_host, R);
@@ -674,7 +691,8 @@ static int verify_attn_impl(const void* q, const void* k_tensormap, const void* 
   memcpy(&kmap, k_tensormap, sizeof(kmap));
   memcpy(&vmap, v_tensormap, sizeof(vmap));
 
-  const AttnPlan plan = attn_plan(R, H, d, kv_len_max);
+  const int rows = R * grp;  // packed rows of one CTA (the launch instance is chosen on these)
+  const AttnPlan plan = attn_plan(rows, H, d, kv_len_max);
   const AttnWorkspace w = attn_workspace(workspace, H, d);
   const int G = plan.G;
   const uint32_t* tab = w.table[plan.table_idx];
@@ -688,11 +706,11 @@ static int verify_attn_impl(const void* q, const void* k_tensormap, const void* 
   const uint32_t pf_chunks = pf_ptr ? (uint32_t)(next_weight_bytes / kPfChunk) : 0u;
 
   if (d == 128) {
-    if (R <= 16) return launch_mma<128, 1, 3>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
-    return launch_mma<128, 2, 6>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
+    if (rows <= 16) return launch_mma<128, 1, 3>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
+    return launch_mma<128, 2, 6>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
   }
-  if (R <= 16) return launch_mma<64, 1, 4>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
-  return launch_mma<64, 2, 4>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
+  if (rows <= 16) return launch_mma<64, 1, 4>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
+  return launch_mma<64, 2, 4>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
 }
 
 // Measures the per-CTA streaming time of this very kernel on the caller's KV store and installs a split table
@@ -738,7 +756,7 @@ int tf_verify_attn_calibrate(const void* q, const void* k_tensormap, const void*
     // per-CTA median of three launches (after one warm-up launch under the new table)
     for (int rep = 0; rep < 4; ++rep) {
       TF_CHECK_CUDA(cudaMemsetAsync(w.cta_ns, 0, (size_t)G * sizeof(uint32_t), stream));
-      const int rc = verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len, nullptr, kv_len, R, H, d, scale, out, workspace,
+      const int rc = verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len, nullptr, kv_len, R, H, 1, d, scale, out, workspace,
                                       workspace_bytes, 0, nullptr, 0, true, 0, stream_);
       if (rc != TF_OK) return rc;
       if (rep > 0) {
@@ -791,8 +809,25 @@ int tf_verify_attn_calibrate(const void* q, const void* k_tensormap, const void*
 int tf_verify_attn(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
                    const int32_t* kv_len_dev, int kv_len_max, int R, int H, int d, float scale, void* out,
                    void* workspace, size_t workspace_bytes, int variant, int clean_keys, tf_stream_t stream) {
-  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, d, scale, out, workspace,
+  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, 1, d, scale, out, workspace,
                           workspace_bytes, variant, nullptr, 0, false, clean_keys, stream);
+}
+
+static int gqa_group(int Hq, int Hkv, const char* what) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0) {
+    tf::set_error("%s: Hq (%d) must be a positive multiple of Hkv (%d)", what, Hq, Hkv);
+    return 0;
+  }
+  return Hq / Hkv;
+}
+
+int tf_verify_attn_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
+                       const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv, int d, float scale, void* out,
+                       void* workspace, size_t workspace_bytes, int variant, int clean_keys, tf_stream_t stream) {
+  const int grp = gqa_group(Hq, Hkv, "tf_verify_attn_gqa");
+  if (grp == 0) return TF_ERR_INVALID;
+  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hkv, grp, d, scale, out,
+                          workspace, workspace_bytes, variant, nullptr, 0, false, clean_keys, stream);
 }
 
 int tf_verify_attn_prefetch(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
@@ -803,13 +838,14 @@ int tf_verify_attn_prefetch(const void* q, const void* k_tensormap, const void* 
     tf::set_error("tf_verify_attn_prefetch: next_weights must be 16-byte aligned");
     return TF_ERR_INVALID;
   }
-  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, d, scale, out, workspace,
+  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, 1, d, scale, out, workspace,
                           workspace_bytes, variant, nullptr, 0, false, clean_keys, stream, next_weights, next_weight_bytes);
 }
 
-int tf_verify_attn_tree(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
-                        const int32_t* kv_len_dev, int kv_len_max, int R, int H, int d, float scale, const uint32_t* tree_mask,
-                        int tree_cols, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+static int verify_attn_tree_impl(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
+                                 const int32_t* kv_len_dev, int kv_len_max, int R, int H, int grp, int d, float scale,
+                                 const uint32_t* tree_mask, int tree_cols, void* out, void* workspace, size_t workspace_bytes,
+                                 tf_stream_t stream) {
   if (!tree_mask || tree_cols <= 0 || tree_cols % 32 != 0) {
     tf::set_error("tf_verify_attn_tree: tree_mask must be non-NULL and tree_cols a positive multiple of 32 (got %d)", tree_cols);
     return TF_ERR_INVALID;
@@ -818,8 +854,25 @@ int tf_verify_attn_tree(const void* q, const void* k_tensormap, const void* v_te
     tf::set_error("tf_verify_attn_tree: kv_len (%d) must include the %d tree columns", kv_len_host, tree_cols);
     return TF_ERR_INVALID;
   }
-  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, d, scale, out, workspace,
+  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, grp, d, scale, out, workspace,
                           workspace_bytes, 0, tree_mask, tree_cols, false, 0, stream);
+}
+
+int tf_verify_attn_tree(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
+                        const int32_t* kv_len_dev, int kv_len_max, int R, int H, int d, float scale, const uint32_t* tree_mask,
+                        int tree_cols, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  return verify_attn_tree_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, H, 1, d, scale, tree_mask,
+                               tree_cols, out, workspace, workspace_bytes, stream);
+}
+
+int tf_verify_attn_tree_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,
+                            const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv, int d, float scale,
+                            const uint32_t* tree_mask, int tree_cols, void* out, void* workspace, size_t workspace_bytes,
+                            tf_stream_t stream) {
+  const int grp = gqa_group(Hq, Hkv, "tf_verify_attn_tree_gqa");
+  if (grp == 0) return TF_ERR_INVALID;
+  return verify_attn_tree_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hkv, grp, d, scale,
+                               tree_mask, tree_cols, out, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import glob
 import os
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
@@ -42,8 +42,9 @@ def _load_local_checkpoint(path: str) -> Dict[str, torch.Tensor]:
     return sd
 
 
-def shape_from_hf_config(path: str) -> LlamaShape:
-    """`LlamaShape` from an HF checkpoint directory's config.json (the fields the reference reads off `LlamaConfig`)."""
+def shape_from_hf_config(path: str, gqa_retrieval: Optional[str] = None) -> LlamaShape:
+    """`LlamaShape` from an HF checkpoint directory's config.json (the fields the reference reads off `LlamaConfig`).
+    A grouped-query checkpoint needs `gqa_retrieval` (see LlamaShape.gqa_retrieval); without it, it is refused."""
     import json
     with open(os.path.join(path, "config.json")) as f:
         c = json.load(f)
@@ -61,7 +62,7 @@ def shape_from_hf_config(path: str) -> LlamaShape:
                       num_attention_heads=c["num_attention_heads"], num_key_value_heads=c.get("num_key_value_heads"),
                       vocab_size=c["vocab_size"], max_position_embeddings=c.get("max_position_embeddings", 4096),
                       rms_norm_eps=c.get("rms_norm_eps", 1e-5), rope_theta=float(c.get("rope_theta", 10000.0)), rope_scaling=rs,
-                      name=c.get("_name_or_path") or os.path.basename(os.path.normpath(path)))
+                      name=c.get("_name_or_path") or os.path.basename(os.path.normpath(path)), gqa_retrieval=gqa_retrieval)
 
 
 def _device_from_map(device_map) -> torch.device:
@@ -77,16 +78,19 @@ class _Factory:
 
     @classmethod
     def from_pretrained(cls, name_or_path: str, torch_dtype=torch.float16, device_map=None, synthetic=None, seed: int = 0,
-                        config: LlamaShape = None, **kw) -> LlamaModel:
+                        config: LlamaShape = None, gqa_retrieval: Optional[str] = None, **kw) -> LlamaModel:
         if torch_dtype not in (None, torch.float16):
             raise ValueError("the TriForce hot path is fp16 (reference: torch_dtype=torch.float16)")
         is_dir = os.path.isdir(name_or_path)
         if config is not None:
             shape = config
         elif is_dir:  # a local checkpoint: its own config.json describes it (hub ids are resolved by name)
-            shape = shape_from_hf_config(name_or_path)
+            shape = shape_from_hf_config(name_or_path, gqa_retrieval=gqa_retrieval)
         else:
             shape = named_config(_HUB_TO_SHAPE.get(name_or_path, name_or_path))
+        if (gqa_retrieval is not None and shape.num_key_value_heads != shape.num_attention_heads
+                and gqa_retrieval != shape.gqa_retrieval):
+            raise ValueError(f"{name_or_path}: gqa_retrieval={gqa_retrieval!r} conflicts with the shape's rule {shape.gqa_retrieval!r}")
         dev = _device_from_map(device_map)
         if synthetic is None:
             synthetic = os.environ.get("TRIFORCE_SYNTHETIC", "0") == "1"

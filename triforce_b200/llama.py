@@ -35,10 +35,12 @@ class _LayerWeights:
 
 
 def _prefill_attention_library(q, key_layer, value_layer, kv_len: int, scale: float) -> torch.Tensor:
-    """q [n,H,d]; key_layer/value_layer [H,cap,d].  Bottom-right causal attention of n new rows over kv_len keys."""
+    """q [n,H,d]; key_layer/value_layer [Hkv,cap,d] (H % Hkv == 0, query head h reads KV head h // (H/Hkv)).  Bottom-right
+    causal attention of n new rows over kv_len keys."""
     n, H, d = q.shape
+    grp = H // key_layer.shape[0]
     try:
-        from flash_attn import flash_attn_with_kvcache  # library kernel, prefill only
+        from flash_attn import flash_attn_with_kvcache  # library kernel, prefill only; takes GQA natively
         k = key_layer.permute(1, 0, 2)[None, :kv_len]
         v = value_layer.permute(1, 0, 2)[None, :kv_len]
         return flash_attn_with_kvcache(q[None], k, v, softmax_scale=scale, causal=True)[0]
@@ -46,6 +48,8 @@ def _prefill_attention_library(q, key_layer, value_layer, kv_len: int, scale: fl
         qh = q.transpose(0, 1)[None]  # [1,H,n,d]
         k = key_layer[None, :, :kv_len]
         v = value_layer[None, :, :kv_len]
+        if grp > 1:
+            k, v = k.repeat_interleave(grp, dim=1), v.repeat_interleave(grp, dim=1)
         i = torch.arange(n, device=q.device)[:, None]
         j = torch.arange(kv_len, device=q.device)[None, :]
         mask = j <= i + (kv_len - n)
@@ -56,12 +60,17 @@ def _prefill_attention_library(q, key_layer, value_layer, kv_len: int, scale: fl
 def shard_layer_weights(state_dict: Dict[str, torch.Tensor], config: LlamaShape, layer: int, tp_rank: int, tp_world: int,
                         device=None):
     """Megatron-style shard of one decoder layer (reference models/TP_layers.py:126-147): q/k/v/gate/up are split by
-    OUTPUT rows (heads / intermediate columns), o/down by INPUT columns; returns fused (wqkv, wo, wgu, wd)."""
-    H, d = config.num_attention_heads, config.head_dim
+    OUTPUT rows (heads / intermediate columns), o/down by INPUT columns; returns fused (wqkv, wo, wgu, wd).  q rows are
+    sliced by query head and k/v rows by KV head, so wqkv is [Hq·d | Hkv·d | Hkv·d] / world."""
+    H, Hkv, d = config.num_attention_heads, config.num_key_value_heads, config.head_dim
     if H % tp_world or config.intermediate_size % tp_world:
         raise ValueError(f"heads ({H}) and intermediate size ({config.intermediate_size}) must be divisible by world size {tp_world}")
+    if Hkv % tp_world:
+        raise ValueError(f"key/value heads ({Hkv}) must be divisible by world size {tp_world}")
     Hl, Il = H // tp_world, config.intermediate_size // tp_world
     h0, h1 = tp_rank * Hl * d, (tp_rank + 1) * Hl * d
+    Hkvl = Hkv // tp_world
+    k0, k1 = tp_rank * Hkvl * d, (tp_rank + 1) * Hkvl * d
     i0, i1 = tp_rank * Il, (tp_rank + 1) * Il
     p = f"model.layers.{layer}."
 
@@ -69,7 +78,7 @@ def shard_layer_weights(state_dict: Dict[str, torch.Tensor], config: LlamaShape,
         t = state_dict[p + name]
         return t.to(device=device, dtype=torch.float16) if device is not None else t
 
-    wqkv = torch.cat([g("self_attn.q_proj.weight")[h0:h1], g("self_attn.k_proj.weight")[h0:h1], g("self_attn.v_proj.weight")[h0:h1]], 0).contiguous()
+    wqkv = torch.cat([g("self_attn.q_proj.weight")[h0:h1], g("self_attn.k_proj.weight")[k0:k1], g("self_attn.v_proj.weight")[k0:k1]], 0).contiguous()
     wo = g("self_attn.o_proj.weight")[:, h0:h1].contiguous()
     wgu = torch.cat([g("mlp.gate_proj.weight")[i0:i1], g("mlp.up_proj.weight")[i0:i1]], 0).contiguous()
     wd = g("mlp.down_proj.weight")[:, i0:i1].contiguous()
@@ -92,8 +101,11 @@ class LlamaModel:
         H, d = config.num_attention_heads, config.head_dim
         assert H % tp_world == 0, "num_attention_heads must be divisible by the TP world size"
         assert config.intermediate_size % tp_world == 0
+        assert config.num_key_value_heads % tp_world == 0, "num_key_value_heads must be divisible by the TP world size"
         self.local_num_heads = H // tp_world
-        self.local_num_kv_heads = self.local_num_heads
+        self.local_num_kv_heads = config.num_key_value_heads // tp_world
+        self.gqa = self.local_num_kv_heads != self.local_num_heads
+        assert not (self.gqa and is_draft), "the draft is multi-head attention"
         self.head_dim = d
         self.prefill_chunk = prefill_chunk
         Hl, Il = self.local_num_heads, config.intermediate_size // tp_world
@@ -171,8 +183,37 @@ class LlamaModel:
 
     def _workspace(self) -> torch.Tensor:
         if self._attn_ws is None:
-            self._attn_ws = ops.verify_attn_workspace(ops.VERIFY_MAX_ROWS, self.local_num_heads, self.head_dim, self.device)
+            if self.gqa:
+                self._attn_ws = ops.verify_attn_gqa_workspace(self.local_num_heads, self.local_num_kv_heads, self.head_dim, self.device)
+            else:
+                self._attn_ws = ops.verify_attn_workspace(ops.VERIFY_MAX_ROWS, self.local_num_heads, self.head_dim, self.device)
         return self._attn_ws
+
+    # --- attention entry points: MHA, or grouped-query (Hkv < Hq) through the *_gqa kernels -----------------------------
+    def _rope_append(self, qkv, q_out, key_layer, value_layer, **kw):
+        if self.gqa:
+            ops.rope_append_gqa(qkv, self.local_num_heads, self.local_num_kv_heads, self.head_dim, self.cos, self.sin, q_out,
+                                key_layer, value_layer, **kw)
+        else:
+            ops.rope_append(qkv, self.local_num_heads, self.head_dim, self.cos, self.sin, q_out, key_layer, value_layer, **kw)
+
+    def _verify_attn(self, q_out, maps, layer, kv_len, n, out, ws, kv_len_dev=None, clean_keys=0, next_weights=None):
+        Hl, d = self.local_num_heads, self.head_dim
+        if self.gqa:  # no L2 prefetch for GQA launches
+            ops.verify_attn_gqa(q_out, maps, layer, kv_len, n, Hl, self.local_num_kv_heads, d, self.scale, out, ws,
+                                kv_len_dev=kv_len_dev, clean_keys=clean_keys)
+        else:
+            ops.verify_attn(q_out, maps, layer, kv_len, n, Hl, d, self.scale, out, ws, kv_len_dev=kv_len_dev,
+                            variant=self.attn_variant, clean_keys=clean_keys, next_weights=next_weights)
+
+    def _tree_attn_tc(self, q_out, maps, layer, kv_len, n, mask_bits, tree_cols, out, causal=False):
+        Hl, d = self.local_num_heads, self.head_dim
+        ws = self._tc_workspace(n, maps)
+        if self.gqa:
+            ops.tree_attn_tc_gqa(q_out, maps, layer, kv_len, n, Hl, self.local_num_kv_heads, d, self.scale, mask_bits, tree_cols,
+                                 out, ws, causal=causal)
+        else:
+            ops.tree_attn_tc(q_out, maps, layer, kv_len, n, Hl, d, self.scale, mask_bits, tree_cols, out, ws, causal=causal)
 
     def calibrate_attention(self, kv_cache, rows: int = 7, rounds: int = 4) -> Optional[dict]:
         """Init-time load balancing of the verify attention on this GPU (tf_verify_attn_calibrate): the kernel's per-CTA key
@@ -181,7 +222,7 @@ class LlamaModel:
         on an H100 the equal split is faster (full-KV verify at 124 944 keys: 0.684 ms equal vs 0.721-0.726 ms calibrated per
         layer) and, unlike a split measured at start-up, bit-reproducible across processes.  Short stores (< 16K keys) are left
         alone — there is nothing to balance."""
-        if os.environ.get("TRIFORCE_ATTN_CALIBRATE", "0") != "1" or self.is_draft:
+        if os.environ.get("TRIFORCE_ATTN_CALIBRATE", "0") != "1" or self.is_draft or self.gqa:
             return None
         maps = kv_cache.tensor_maps
         cap = int(maps.shape[2])
@@ -310,34 +351,30 @@ class LlamaModel:
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             if spec:
-                ops.rope_append(qkv, Hl, d, self.cos, self.sin, q_out, graph_cache.key_store[l], graph_cache.value_store[l],
-                                pos_ids=pos32, slot0=graph_cache.max_budget)
-                ops.verify_attn(q_out, graph_cache.tensor_maps, l, graph_cache.real_budget, n, Hl, d, self.scale, out, ws,
-                                variant=self.attn_variant, clean_keys=graph_cache.max_budget,  # rope_append wrote slots >= budget only
-                                next_weights=self.layers[l].wo if self.attn_prefetch else None)  # o_proj's weights ride into L2
+                self._rope_append(qkv, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
+                                  slot0=graph_cache.max_budget)
+                self._verify_attn(q_out, graph_cache.tensor_maps, l, graph_cache.real_budget, n, out, ws,
+                                  clean_keys=graph_cache.max_budget,  # rope_append wrote slots >= budget only
+                                  next_weights=self.layers[l].wo if self.attn_prefetch else None)  # o_proj's weights ride into L2
                 return out
             if use_device_len:
-                ops.rope_append(qkv, Hl, d, self.cos, self.sin, q_out, kv_cache.key_store[l], kv_cache.value_store[l],
-                                pos0_dev=kv_cache.seq_len_dev, slot0_dev=kv_cache.seq_len_dev)
-                ops.verify_attn(q_out, kv_cache.tensor_maps, l, n, n, Hl, d, self.scale, out, ws,
-                                kv_len_dev=kv_cache.seq_len_dev, variant=self.attn_variant)
+                self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos0_dev=kv_cache.seq_len_dev,
+                                  slot0_dev=kv_cache.seq_len_dev)
+                self._verify_attn(q_out, kv_cache.tensor_maps, l, n, n, out, ws, kv_len_dev=kv_cache.seq_len_dev)
                 return out
             if position_ids is not None:
-                ops.rope_append(qkv, Hl, d, self.cos, self.sin, q_out, kv_cache.key_store[l], kv_cache.value_store[l],
-                                pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=old_len)
+                self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l],
+                                  pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=old_len)
             else:
-                ops.rope_append(qkv, Hl, d, self.cos, self.sin, q_out, kv_cache.key_store[l], kv_cache.value_store[l],
-                                pos0=old_len, slot0=old_len)
+                self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos0=old_len, slot0=old_len)
             if build:
                 qs[l] = q_out[0]
             if n <= ops.VERIFY_MAX_ROWS:
-                ops.verify_attn(q_out, kv_cache.tensor_maps, l, old_len + n, n, Hl, d, self.scale, out, ws,
-                                variant=self.attn_variant)
+                self._verify_attn(q_out, kv_cache.tensor_maps, l, old_len + n, n, out, ws)
                 return out
             if d == 128 and self.prefill_tc:
                 # prompt chunks on the wgmma kernel in causal mode (SURVEY §8 row f-2): no library call on the 7B / 13B path
-                ops.tree_attn_tc(q_out, kv_cache.tensor_maps, l, old_len + n, n, Hl, d, self.scale, None, 0, out,
-                                 self._tc_workspace(n, kv_cache.tensor_maps), causal=True)
+                self._tree_attn_tc(q_out, kv_cache.tensor_maps, l, old_len + n, n, None, 0, out, causal=True)
                 return out
             return _prefill_attention_library(q_out, kv_cache.key_store[l], kv_cache.value_store[l], old_len + n, self.scale)
 
@@ -366,9 +403,13 @@ class LlamaModel:
         if d == 128 and n >= 128 and n % 128 == 0 and os.environ.get("TRIFORCE_TREE_TC", "1") == "1":
             # the whole tree in ONE pass over the KV on the tensor cores (wgmma, variant 2; reads each KV byte n/128 times
             # instead of n/32 times)
-            ops.tree_attn_tc(q_out, maps, layer, kv_len, n, Hl, d, self.scale, mask_bits, tree_cols, out, self._tc_workspace(n, maps))
+            self._tree_attn_tc(q_out, maps, layer, kv_len, n, mask_bits, tree_cols, out)
             return
         ws = self._workspace()
+        if self.gqa:  # blocks of VERIFY_MAX_ROWS / group-size rows (ops.verify_attn_gqa)
+            ops.verify_attn_gqa(q_out, maps, layer, kv_len, n, Hl, self.local_num_kv_heads, d, self.scale, out, ws,
+                                tree_mask=mask_bits[:n], tree_cols=tree_cols)
+            return
         for r0 in range(0, n, ops.VERIFY_MAX_ROWS):
             r1 = min(n, r0 + ops.VERIFY_MAX_ROWS)
             ops.verify_attn_tree(q_out[r0:r1], maps, layer, kv_len, r1 - r0, Hl, d, self.scale, mask_bits[r0:r1], tree_cols,
@@ -386,8 +427,8 @@ class LlamaModel:
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-            ops.rope_append(qkv, Hl, d, self.cos, self.sin, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
-                            slot0=graph_cache.max_budget + storage_start)
+            self._rope_append(qkv, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
+                              slot0=graph_cache.max_budget + storage_start)
             self._tree_attention(q_out, graph_cache.tensor_maps, l, graph_cache.real_budget, mask_bits, T, out)
             return out
 
@@ -405,8 +446,7 @@ class LlamaModel:
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-            ops.rope_append(qkv, Hl, d, self.cos, self.sin, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos_ids=pos32,
-                            slot0=old_len)
+            self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos_ids=pos32, slot0=old_len)
             self._tree_attention(q_out, kv_cache.tensor_maps, l, old_len + T, mask_bits, T, out)
             return out
 

@@ -70,6 +70,30 @@ def retrieval_build(key_store, value_store, q, retr_key_store, retr_value_store,
     COUNTER.n += 3
 
 
+def retrieval_build_gqa(key_store, value_store, q, retr_key_store, retr_value_store, prefill: int, chunk: int, budget: int,
+                        layer0: int = 0, n_layers: Optional[int] = None, out_idx=None, out_scores=None):
+    """retrieval_build for a grouped-query target under the "group_sum" rule (tf_retrieval_build_gqa): stores [L,Hkv,cap,d];
+    q [n_layers,Hq,d]; out_idx [n,Hkv,budget/chunk]; out_scores [n,Hkv,prefill/chunk]."""
+    require_cuda(key_store, value_store, q, retr_key_store, retr_value_store)
+    L, Hkv, cap, d = key_store.shape
+    n = q.shape[0] if n_layers is None else n_layers
+    Hq = q.shape[1]
+    _f16c(q, "q")
+    assert q.is_contiguous() and q.shape == (n, Hq, d), (q.shape, (n, Hq, d))
+    ws_bytes = lib().tf_retrieval_build_workspace_bytes(n, Hkv, d, prefill, chunk, budget)
+    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=q.device)
+    if out_idx is not None:
+        assert out_idx.dtype == torch.int32 and out_idx.is_contiguous() and out_idx.shape == (n, Hkv, budget // chunk)
+    if out_scores is not None:
+        assert out_scores.dtype == torch.float16 and out_scores.is_contiguous() and out_scores.shape == (n, Hkv, prefill // chunk)
+    check(lib().tf_retrieval_build_gqa(key_store[layer0].data_ptr(), value_store[layer0].data_ptr(), key_store.stride(0),
+                                       key_store.stride(1), q.data_ptr(), n, Hq, Hkv, d, prefill, chunk, budget,
+                                       retr_key_store[layer0].data_ptr(), retr_value_store[layer0].data_ptr(),
+                                       retr_key_store.stride(0), retr_key_store.stride(1), ptr(out_idx), ptr(out_scores),
+                                       ws.data_ptr(), ws.numel(), stream_ptr()), "tf_retrieval_build_gqa")
+    COUNTER.n += 3
+
+
 def rope_append(qkv: torch.Tensor, H: int, d: int, cos, sin, q_out, key_layer, value_layer, *, pos_ids=None, pos0: int = 0,
                 pos0_dev=None, slot0: int = 0, slot0_dev=None, rotate_q=True, rotate_k=True):
     """qkv [R, 3*H*d] (q|k|v); key_layer/value_layer [H,cap,d] of one layer; q_out [R,H,d]."""
@@ -86,6 +110,26 @@ def rope_append(qkv: torch.Tensor, H: int, d: int, cos, sin, q_out, key_layer, v
                                cos.shape[0], ptr(pos_ids), pos0, ptr(pos0_dev), slot0, ptr(slot0_dev), R, H, d,
                                int(rotate_q), int(rotate_k), q_out.data_ptr(), key_layer.data_ptr(), value_layer.data_ptr(),
                                key_layer.stride(0), key_layer.shape[1], stream_ptr()), "tf_rope_append")
+    COUNTER.n += 1
+
+
+def rope_append_gqa(qkv: torch.Tensor, Hq: int, Hkv: int, d: int, cos, sin, q_out, key_layer, value_layer, *, pos_ids=None,
+                    pos0: int = 0, pos0_dev=None, slot0: int = 0, slot0_dev=None):
+    """qkv [R, (Hq + 2 Hkv) d] (q|k|v); key_layer/value_layer [Hkv,cap,d] of one layer; q_out [R,Hq,d] (tf_rope_append_gqa)."""
+    require_cuda(qkv, cos, sin, q_out, key_layer, value_layer)
+    _f16c(qkv, "qkv")
+    R = qkv.shape[0]
+    assert qkv.stride(1) == 1 and qkv.shape[1] == (Hq + 2 * Hkv) * d
+    assert q_out.is_contiguous() and q_out.shape == (R, Hq, d) and key_layer.stride(2) == 1 and key_layer.stride(1) == d
+    assert key_layer.shape[0] == Hkv
+    base = qkv.data_ptr()
+    es = qkv.element_size()
+    if pos_ids is not None:
+        assert pos_ids.dtype == torch.int32 and pos_ids.numel() >= R
+    check(lib().tf_rope_append_gqa(base, base + Hq * d * es, base + (Hq + Hkv) * d * es, qkv.stride(0), cos.data_ptr(),
+                                   sin.data_ptr(), cos.shape[0], ptr(pos_ids), pos0, ptr(pos0_dev), slot0, ptr(slot0_dev), R, Hq,
+                                   Hkv, d, 1, 1, q_out.data_ptr(), key_layer.data_ptr(), value_layer.data_ptr(),
+                                   key_layer.stride(0), key_layer.shape[1], stream_ptr()), "tf_rope_append_gqa")
     COUNTER.n += 1
 
 
@@ -151,6 +195,54 @@ def verify_attn_tree(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, H: 
     COUNTER.n += 1
 
 
+def verify_attn_gqa_workspace(Hq: int, Hkv: int, d: int, device) -> torch.Tensor:
+    n = lib().tf_verify_attn_gqa_workspace_bytes(VERIFY_MAX_ROWS, Hq, Hkv, d)
+    if n == 0:
+        raise ValueError(f"no verify-attention workspace for Hq={Hq}, Hkv={Hkv}, d={d}")
+    return torch.zeros(n, dtype=torch.uint8, device=device)  # the per-KV-head arrival counters must start at zero
+
+
+def gqa_row_block(Hq: int, Hkv: int) -> int:
+    """Token rows per tf_verify_attn_gqa launch: a CTA holds the rows of a whole query-head group, at most VERIFY_MAX_ROWS."""
+    return VERIFY_MAX_ROWS // (Hq // Hkv)
+
+
+def verify_attn_gqa(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float, out,
+                    workspace, kv_len_dev=None, kv_len_max: Optional[int] = None, clean_keys: int = 0, tree_mask=None,
+                    tree_cols: int = 0):
+    """Verify attention of R token rows of Hq query heads over the Hkv-head store `maps` (tf_verify_attn_gqa, or
+    tf_verify_attn_tree_gqa with `tree_mask` [R, tree_cols/32] over token rows).  The rows are cut into blocks of
+    gqa_row_block(Hq, Hkv) token rows; block [r0, r1) sees kv_len - (R - r1) keys, which keeps it bottom-right aligned in
+    causal mode.  Tree blocks keep kv_len (the tree columns are the last keys) and take their own rows of the mask."""
+    require_cuda(q, out, workspace)
+    _f16c(q, "q")
+    assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and out.shape == q.shape
+    assert maps.shape[1] == Hkv, (maps.shape, Hkv)
+    cap = maps.shape[2]
+    if kv_len_max is None:
+        kv_len_max = cap if kv_len_dev is not None else kv_len
+    if tree_mask is not None:
+        assert tree_mask.is_contiguous() and tree_mask.element_size() == 4 and tree_mask.shape == (R, tree_cols // 32)
+    step = gqa_row_block(Hq, Hkv)
+    if step < 1:
+        raise ValueError(f"{Hq // Hkv} query heads per KV head exceed the {VERIFY_MAX_ROWS} rows of a verify-attention CTA")
+    for r0 in range(0, R, step):
+        r1 = min(R, r0 + step)
+        shift = R - r1  # rows after this block: their keys are not visible to it
+        if tree_mask is None:
+            check(lib().tf_verify_attn_gqa(q[r0:r1].data_ptr(), maps.k_ptr, maps.v_ptr, layer, kv_len - shift, ptr(kv_len_dev),
+                                           min(kv_len_max, cap), r1 - r0, Hq, Hkv, d, scale, out[r0:r1].data_ptr(),
+                                           workspace.data_ptr(), workspace.numel(), 0, clean_keys, stream_ptr()),
+                  "tf_verify_attn_gqa")
+        else:
+            check(lib().tf_verify_attn_tree_gqa(q[r0:r1].data_ptr(), maps.k_ptr, maps.v_ptr, layer, kv_len, ptr(kv_len_dev),
+                                                min(kv_len_max, cap), r1 - r0, Hq, Hkv, d, scale, tree_mask[r0:r1].data_ptr(),
+                                                tree_cols, out[r0:r1].data_ptr(), workspace.data_ptr(), workspace.numel(),
+                                                stream_ptr()),
+                  "tf_verify_attn_tree_gqa")
+        COUNTER.n += 1
+
+
 def tree_attn_tc_workspace(R: int, H: int, kv_len_max: int, device) -> torch.Tensor:
     return torch.empty(lib().tf_tree_attn_tc_workspace_bytes(R, H, kv_len_max), dtype=torch.uint8, device=device)
 
@@ -170,6 +262,21 @@ def tree_attn_tc(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, H: int,
                                 tree_cols, 1 if causal else 0, out.data_ptr(), workspace.data_ptr(), workspace.numel(), ptr(debug_scores),
                                 stream_ptr()),
           "tf_tree_attn_tc")
+    COUNTER.n += 2
+
+
+def tree_attn_tc_gqa(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float,
+                     tree_mask: Optional[torch.Tensor], tree_cols: int, out, workspace, causal: bool = False):
+    """tree_attn_tc for Hq query heads over the Hkv-head store `maps` (tf_tree_attn_tc_gqa); workspace from
+    tree_attn_tc_workspace(R, Hq, kv_len_max)."""
+    require_cuda(q, out, workspace)
+    _f16c(q, "q")
+    assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and maps.shape[1] == Hkv
+    if tree_cols:
+        assert tree_mask is not None and tree_mask.is_contiguous() and tree_mask.element_size() == 4 and tree_mask.numel() >= R * (tree_cols // 32)
+    check(lib().tf_tree_attn_tc_gqa(q.data_ptr(), maps.k_ptr, maps.v_ptr, layer, kv_len, R, Hq, Hkv, d, scale,
+                                    ptr(tree_mask) if tree_cols else None, tree_cols, 1 if causal else 0, out.data_ptr(),
+                                    workspace.data_ptr(), workspace.numel(), stream_ptr()), "tf_tree_attn_tc_gqa")
     COUNTER.n += 2
 
 

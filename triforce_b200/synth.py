@@ -20,12 +20,13 @@ from .config import LlamaShape
 
 def _param_shapes(cfg: LlamaShape):
     h, i, v = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
+    hkv = cfg.num_key_value_heads * cfg.head_dim  # == h for MHA
     yield "model.embed_tokens.weight", (v, h), "normal"
     for l in range(cfg.num_hidden_layers):
         p = f"model.layers.{l}."
         yield p + "self_attn.q_proj.weight", (h, h), "normal"
-        yield p + "self_attn.k_proj.weight", (h, h), "normal"
-        yield p + "self_attn.v_proj.weight", (h, h), "normal"
+        yield p + "self_attn.k_proj.weight", (hkv, h), "normal"
+        yield p + "self_attn.v_proj.weight", (hkv, h), "normal"
         yield p + "self_attn.o_proj.weight", (h, h), "normal"
         yield p + "mlp.gate_proj.weight", (i, h), "normal"
         yield p + "mlp.up_proj.weight", (i, h), "normal"

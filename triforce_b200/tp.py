@@ -245,7 +245,7 @@ class DistributedLlama:
         self.num_heads = self.config.num_attention_heads
         self.head_dim = self.config.head_dim
         self.local_num_heads = self.num_heads // world_size
-        self.local_num_key_value_heads = self.local_num_heads
+        self.local_num_key_value_heads = self.config.num_key_value_heads // world_size
         self.model: Optional[LlamaModel] = None
         self.graph_engine: Optional[GraphInferenceEngine] = None
         self.kv_cache = self.retrieval_cache = None
