@@ -53,6 +53,51 @@ int tf_set_pdl(int mask);
 int tf_kv_tensormap_encode(void* out_tensormap_128B, const void* base, int d, long long cap, int heads, int layers,
                            long long head_stride, long long layer_stride, int box_keys);
 
+/* ---- E4M3 full-KV store (opt-in; fp16 stays the default) -----------------------------------------------------------
+ * A store of L layers, Hkv KV heads and `cap` slots is, for K and for V:
+ *   codes     uint8 [L][Hkv][cap][d] (torch.float8_e4m3fn bits), head-major like the fp16 store, strides in bytes;
+ *   exponents int8  [L][Hkv][cap], one per row (the code strides divided by d).
+ * Row x (d fp16 values: K after RoPE, or V): e = the smallest integer with max|x| <= 448 * 2^e (0 for an all-zero row; in
+ * [-32, 8] for finite fp16 x); code = e4m3_rn(x / 2^e), round to nearest even (exact division, nothing saturates).  The row
+ * the store holds is D = fp16_rn(code * 2^e).  Every entry below that reads the store computes what its fp16 counterpart
+ * computes on D; the retrieval cache it fills stays fp16.  Entries take Hq, Hkv (Hq == Hkv is MHA).
+ * tf_kv_tensormap_encode_e4m3: tf_kv_tensormap_encode over a code store (box = one row of d bytes x box_keys rows,
+ *   SWIZZLE_128B at d = 128, SWIZZLE_64B at d = 64); strides in bytes.
+ * tf_kv_quantize_e4m3: fp16 rows [slot0, slot0 + n) of one layer (`src` [Hkv][..][d], head stride in elements, >= cap*d)
+ *   -> the same slots of one layer's codes [Hkv][cap][d] and exponents [Hkv][cap].
+ * tf_rope_append_e4m3: tf_rope_append_gqa (rotate_q = rotate_k = 1; same position, slot and *_dev arguments, same PDL bit 4)
+ *   with the appended K and V rows stored into one layer's codes [Hkv][cap][d] and exponents [Hkv][cap]; q_out is bit-identical.
+ * tf_verify_attn_e4m3: tf_verify_attn_gqa over an E4M3 store (tensor maps from tf_kv_tensormap_encode_e4m3 with box_keys =
+ *   TF_VERIFY_BOX_KEYS; exponents [L][Hkv][cap], 16-byte aligned; cap % TF_VERIFY_BOX_KEYS == 0).  Same stream-K split,
+ *   in-kernel merge, device-side length, R·G packing and workspace (tf_verify_attn_gqa_workspace_bytes).  No calibrated split,
+ *   no L2 prefetch, no tree mode.  V is dequantized exactly to D before the PV product; K enters as (q·code)·2^e in fp32, which is
+ *   q·D exactly unless D rounds: for e < -15 codes below fp16's subnormal step, and a row holding ±65504 (code 256 at e = 8,
+ *   D = ±inf, where this kernel keeps finite scores).  Otherwise results equal the fp16 kernel's on D up to the order of fp32
+ *   sums.
+ * tf_retrieval_build_e4m3: tf_retrieval_build_gqa (Hq == Hkv: tf_retrieval_build) over an E4M3 store; indices, scores and the
+ *   gathered fp16 rows are bit-identical to that build run on D.
+ * tf_tail_update_e4m3: tf_tail_update from an E4M3 store into the fp16 retrieval cache (writes D).
+ */
+int tf_kv_tensormap_encode_e4m3(void* out_tensormap_128B, const void* base, int d, long long cap, int heads, int layers,
+                                long long head_stride, long long layer_stride, int box_keys);
+int tf_kv_quantize_e4m3(const void* src, long long src_head_stride, int slot0, int n, int Hkv, int d, void* codes, int8_t* exps,
+                        long long cap, tf_stream_t stream);
+int tf_rope_append_e4m3(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
+                        int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
+                        const int32_t* slot0_dev, int R, int Hq, int Hkv, int d, void* q_out, void* Kcodes, void* Vcodes,
+                        int8_t* Kexp, int8_t* Vexp, long long cap, tf_stream_t stream);
+int tf_verify_attn_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                        long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv,
+                        int d, float scale, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream);
+int tf_retrieval_build_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                            long long kv_head_stride, const void* q, int n_layers, int Hq, int Hkv, int d, int prefill, int chunk,
+                            int budget, void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride, int32_t* out_idx,
+                            void* out_scores, void* workspace, size_t workspace_bytes, tf_stream_t stream);
+int tf_tail_update_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                        long long kv_head_stride, void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride,
+                        int n_layers, int H, int d, int prefill, int budget, int seq_len_host, const int32_t* seq_len_dev,
+                        int max_new, tf_stream_t stream);
+
 /* ---- (i) retrieval-cache build ---------------------------------------------------------------------------------
  * replaces models/cache.py:154-175 (RetrievalCache.init_graph_cache: ATen mean + cuBLAS bmm + ATen topk + 2 gathers;
  * TP twins :418-453, :517-556).  For each of `n_layers` layers and each head: k̄ = fp16(mean of each `chunk` rows of

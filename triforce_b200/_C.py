@@ -24,6 +24,18 @@ _SIGNATURES = {
     "tf_set_pdl": (c_int, [c_int]),
     "tf_sm_count": (c_int, []),
     "tf_kv_tensormap_encode": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_int, c_longlong, c_longlong, c_int]),
+    "tf_kv_tensormap_encode_e4m3": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_int, c_int, c_longlong, c_longlong, c_int]),
+    "tf_kv_quantize_e4m3": (c_int, [c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_longlong, c_void_p]),
+    "tf_rope_append_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                    c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_longlong, c_void_p]),
+    "tf_verify_attn_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_void_p, c_int, c_int,
+                                    c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tf_retrieval_build_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int,
+                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p,
+                                        c_void_p, c_size_t, c_void_p]),
+    "tf_tail_update_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_longlong,
+                                    c_longlong, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "tf_retrieval_build_workspace_bytes": (c_size_t, [c_int] * 6),
     "tf_retrieval_build": (c_int, [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                    c_int, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,

@@ -63,15 +63,43 @@ class _GatherMixin:
         self.seq_len = offset + len(indices)
 
 
-class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
-    """Full KV of the target (reference cache.py:20-61)."""
+KV_DTYPES = ("fp16", "e4m3")
 
-    def __init__(self, model, max_budget=1024) -> None:
+
+def kv_dtype_of(cache) -> str:
+    return getattr(cache, "kv_dtype", "fp16")
+
+
+def require_fp16_store(cache, what: str) -> None:
+    if kv_dtype_of(cache) != "fp16":
+        raise NotImplementedError(f"{what} needs an fp16 full-KV store; this one is {kv_dtype_of(cache)}")
+
+
+class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
+    """Full KV of the target (reference cache.py:20-61).
+
+    kv_dtype="e4m3" stores the full KV in FP8 E4M3 with one power-of-two exponent per (layer, KV head, slot) row
+    (include/triforce_b200.h): `e4m3` holds codes and exponents, `key_store` / `value_store` are the uint8 codes and the slot
+    count is rounded up to a multiple of 64.  Every kernel reading it computes what its fp16 counterpart computes on the
+    dequantized rows, so the target's numerics change with the store."""
+
+    def __init__(self, model, max_budget=1024, kv_dtype: str = "fp16") -> None:
+        if kv_dtype not in KV_DTYPES:
+            raise ValueError(f"kv_dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
+        self.kv_dtype = kv_dtype
         self.seq_len = 0
         self.max_budget = max_budget
         L, H, d = _model_geometry(model)
         self.hidden_size = model.config.hidden_size
-        self._alloc(L, H, max_budget, d, model.device)
+        self.e4m3: Optional[ops.E4m3Store] = None
+        if kv_dtype == "e4m3":
+            slots = -(-max_budget // ops.VERIFY_BOX_KEYS) * ops.VERIFY_BOX_KEYS
+            self.e4m3 = ops.E4m3Store.empty(L, H, slots, d, model.device)
+            self.key_store, self.value_store = self.e4m3.k_codes, self.e4m3.v_codes
+            self.layers, self.num_heads, self.head_dim, self.slots = L, H, d, slots
+            self._maps = self.e4m3
+        else:
+            self._alloc(L, H, max_budget, d, model.device)
         self.seq_len_dev = torch.zeros(1, dtype=torch.int32, device=model.device)
         self._dev_mirror = 0  # value `seq_len_dev` holds once everything enqueued so far has run
         self.scores = []
@@ -83,6 +111,13 @@ class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
         self.seq_len = 0
         self.key_store.zero_()
         self.value_store.zero_()
+        if self.e4m3 is not None:
+            self.e4m3.k_exp.zero_()
+            self.e4m3.v_exp.zero_()
+
+    def gather_kv_incremental(self, indices, offset: int):
+        require_fp16_store(self, "gather_kv_incremental")
+        super().gather_kv_incremental(indices, offset)
 
     def sync_seq_len_to_device(self):
         """Mirror the Python `seq_len` into `seq_len_dev` on the current stream (graphs read kv_len from there).
@@ -100,6 +135,7 @@ class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
     def update(self, key_states, value_states, layer_idx):
         """Reference-compatible append (cache.py:46-61): key_states [1, n, H, d].  The engine's own forward appends
         through the fused RoPE kernel instead; this exists for API parity."""
+        require_fp16_store(self, "FlashSimpleCache.update")
         n = key_states.shape[-3]
         self.key_cache[layer_idx][:, self.seq_len:self.seq_len + n] = key_states
         self.value_cache[layer_idx][:, self.seq_len:self.seq_len + n] = value_states
@@ -140,25 +176,36 @@ class RetrievalCache(_HeadMajorStore):
         """Per-layer build (cache.py:146-178).  query_states: [1, 1, H, d] post-RoPE query of the last prompt token."""
         assert 1 == query_states.shape[1], "query_states should be 1 for init"
         q = query_states.reshape(1, -1, self.head_dim).contiguous()
-        build = ops.retrieval_build if q.shape[1] == self.num_heads else ops.retrieval_build_gqa  # GQA: the "group_sum" rule
-        build(kv_cache.key_store, kv_cache.value_store, q, self.key_store, self.value_store, self.prefill,
-                            self.chunk_size, self.max_budget, layer0=layer_idx, n_layers=1,
-                            out_idx=self.topk_idx[layer_idx:layer_idx + 1], out_scores=self.chunk_scores[layer_idx:layer_idx + 1])
+        self._build(kv_cache, q, layer_idx, 1)
         if layer_idx == self.layers - 1:
             self.init_graph = True
+
+    def _build(self, kv_cache: FlashSimpleCache, q: torch.Tensor, layer0: int, n: int):
+        out = dict(layer0=layer0, n_layers=n, out_idx=self.topk_idx[layer0:layer0 + n], out_scores=self.chunk_scores[layer0:layer0 + n])
+        if kv_dtype_of(kv_cache) == "e4m3":  # MHA, or GQA under the "group_sum" rule, over the E4M3 store
+            ops.retrieval_build_e4m3(kv_cache.e4m3, q, self.key_store, self.value_store, self.prefill, self.chunk_size,
+                                     self.max_budget, **out)
+            return
+        build = ops.retrieval_build if q.shape[1] == self.num_heads else ops.retrieval_build_gqa  # GQA: the "group_sum" rule
+        build(kv_cache.key_store, kv_cache.value_store, q, self.key_store, self.value_store, self.prefill, self.chunk_size,
+              self.max_budget, **out)
 
     def build_all_layers(self, kv_cache: FlashSimpleCache, queries: torch.Tensor):
         """All layers in ONE launch sequence (3 kernels instead of 3*L): `queries` [L, H, d].  The selection of layer l
         only needs that layer's query and full K, both final once the last prompt token has gone through layer l.
         A grouped-query target passes its Hq query heads and is scored by the "group_sum" rule (tf_retrieval_build_gqa)."""
-        build = ops.retrieval_build if queries.shape[1] == self.num_heads else ops.retrieval_build_gqa
-        build(kv_cache.key_store, kv_cache.value_store, queries.contiguous(), self.key_store, self.value_store,
-                            self.prefill, self.chunk_size, self.max_budget, layer0=0, n_layers=self.layers,
-                            out_idx=self.topk_idx, out_scores=self.chunk_scores)
+        self._build(kv_cache, queries.contiguous(), 0, self.layers)
         self.init_graph = True
 
     def update_graph_cache(self, kv_cache: Optional[FlashSimpleCache] = None, use_device_len: bool = False, max_new: int = 0):
         """cache.py:180-182: KV of every committed generated token overwrites the budget tail, all layers."""
+        if kv_dtype_of(kv_cache) == "e4m3":  # the dequantized rows of the E4M3 store
+            if use_device_len:
+                ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, 0,
+                                     kv_cache.seq_len_dev, max_new)
+            else:
+                ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, kv_cache.seq_len)
+            return
         if use_device_len:
             ops.tail_update(kv_cache.key_store, kv_cache.value_store, self.key_store, self.value_store, self.prefill,
                             self.max_budget, 0, kv_cache.seq_len_dev, max_new)
@@ -177,7 +224,10 @@ class RetrievalCache(_HeadMajorStore):
         `init_graph` set)."""
         self.init_graph_cache(kv_cache, query_states, layer_idx)
         n = kv_cache.seq_len - self.prefill
-        if n > 0:
+        if n > 0 and kv_dtype_of(kv_cache) == "e4m3":
+            ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, kv_cache.seq_len,
+                                 layer0=layer_idx, n_layers=1)
+        elif n > 0:
             self.key_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.key_store[layer_idx, :, self.prefill:kv_cache.seq_len]
             self.value_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.value_store[layer_idx, :, self.prefill:kv_cache.seq_len]
 
@@ -196,6 +246,7 @@ class RetrievalCacheSeqouia(RetrievalCache):
         assert self.real_budget == max_budget + tree_size
 
     def init_graph_cache(self, kv_cache, query_states, layer_idx):
+        require_fp16_store(kv_cache, "the Sequoia retrieval cache")
         if self.init_graph:
             raise ValueError("Graph is already initialized")  # cache.py:420-421
         super().init_graph_cache(kv_cache, query_states, layer_idx)

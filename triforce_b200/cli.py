@@ -51,6 +51,8 @@ FLAGS = {
         ("--target_path", dict(type=str, default=None, help="local HF checkpoint dir of the target")),
         ("--draft_path", dict(type=str, default=None, help="local HF checkpoint dir of the draft")),
         ("--seed", dict(type=int, default=0)),
+        ("--kv_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
+                            help="full-KV store: fp16, or FP8 E4M3 with a per-row power-of-two scale (changes the target's numerics)")),
     ],
     "offloading_TP": _COMMON_TP_FLAGS + [("--gamma", dict(type=str, default=6))],
     "offloading_seqouia": _COMMON_TP_FLAGS + [("--tree_size", dict(type=str, default="512"))],
@@ -128,7 +130,7 @@ def run_on_chip(argv: Optional[List[str]] = None) -> None:
                  spec_args={"budget": args.budget, "chunk_size": args.chunk_size}, dataset=args.dataset)
 
     # caches and engine (on_chip.py:76-83)
-    cache = FlashSimpleCache(target, prefill + gen_len + 16)
+    cache = FlashSimpleCache(target, prefill + gen_len + 16, kv_dtype=args.kv_dtype)
     graph_cache = RetrievalCache(target, max_budget=args.budget, prefill=prefill, gamma=gamma, chunk_size=args.chunk_size)
     draft_cache = StreamingLLMEvictionCache(draft, start_size=16, recent_size=args.draft_cache_budget - 16 - gamma, gamma=gamma)
     engine = GraphInferenceEngine(target, cache, graph_cache, draft, draft_cache)

@@ -141,4 +141,54 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
+// ---- E4M3 full-KV store ---------------------------------------------------------------------------------------------
+// A row x of d fp16 values (K after RoPE, or V) of one (layer, KV head, slot) is stored as one int8 exponent e and d codes
+//   e    = the smallest integer with max|x| <= 448 * 2^e (0 for an all-zero row; in [-32, 8] for finite fp16 input),
+//   code = e4m3_rn(x / 2^e)   (round to nearest even; x / 2^e is exact and |x / 2^e| <= 448, so nothing saturates).
+// The row the store stands for is D = fp16_rn(code * 2^e).  Every kernel that reads the store computes what its fp16
+// counterpart computes on D; tests/kv_e4m3_oracle.py restates the rule.  These functions are the only place it is coded.
+__device__ __forceinline__ int kv_e4m3_exponent(float amax) {
+  if (!(amax > 0.f)) return 0;
+  const uint32_t b = __float_as_uint(amax);  // amax = 1.m * 2^E; 448 = 1.75 * 2^8
+  const int E = (int)(b >> 23) - 127;
+  return (b & 0x7fffffu) <= 0x600000u ? E - 8 : E - 7;
+}
+__device__ __forceinline__ float kv_e4m3_pow2(int e) { return __uint_as_float((uint32_t)(e + 127) << 23); }
+// codes of (lo, hi) at exponent e: lo in the low byte
+__device__ __forceinline__ uint16_t kv_e4m3_quantize2(float lo, float hi, int e) {
+  const float s = kv_e4m3_pow2(-e);
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi * s), "f"(lo * s));
+  return r;
+}
+// two codes (lo in the low byte) -> their exact fp16 values
+__device__ __forceinline__ __half2 kv_e4m3_codes2(uint16_t c) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(c));
+  return *reinterpret_cast<__half2*>(&r);
+}
+// D = fp16_rn(fp16_rn(c * a) * b) with (a, b) = (1, 2^e), or (2^-8, 2^(e+8)) below e = -24 where 2^e has no fp16: the
+// first product is exact (codes are multiples of 2^-9), so D is rounded once
+__device__ __forceinline__ void kv_e4m3_factors(int e, __half& a, __half& b) {
+  a = __float2half_rn(e < -24 ? 0.00390625f : 1.f);
+  b = __float2half_rn(kv_e4m3_pow2(e < -24 ? e + 8 : e));
+}
+__device__ __forceinline__ __half2 kv_e4m3_apply(__half2 c, __half2 a, __half2 b) { return __hmul2_rn(__hmul2_rn(c, a), b); }
+// two codes of one row (exponent e) -> D
+__device__ __forceinline__ __half2 kv_e4m3_dequant2(uint16_t c, int e) {
+  __half a, b;
+  kv_e4m3_factors(e, a, b);
+  return kv_e4m3_apply(kv_e4m3_codes2(c), __half2half2(a), __half2half2(b));
+}
+// 8 codes of one row -> 8 fp16 values of D
+__device__ __forceinline__ uint4 kv_e4m3_dequant8(uint2 c, int e) {
+  uint4 r;
+  __half2* o = reinterpret_cast<__half2*>(&r);
+  o[0] = kv_e4m3_dequant2((uint16_t)(c.x & 0xffffu), e);
+  o[1] = kv_e4m3_dequant2((uint16_t)(c.x >> 16), e);
+  o[2] = kv_e4m3_dequant2((uint16_t)(c.y & 0xffffu), e);
+  o[3] = kv_e4m3_dequant2((uint16_t)(c.y >> 16), e);
+  return r;
+}
+
 }  // namespace tf

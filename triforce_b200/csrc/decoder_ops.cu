@@ -14,7 +14,28 @@ __device__ __forceinline__ void rope_pair(__half2 a, __half2 b, __half2 cos_lo, 
   out_hi = __hadd2_rn(__hmul2_rn(b, cos_hi), __hmul2_rn(a, sin_hi));
 }
 
+// the amax of a row held by the D/4 threads of a rope_append CTA (one warp at d = 128, half a warp at d = 64)
 template <int D>
+__device__ __forceinline__ float row_amax(__half2 lo, __half2 hi) {
+  const __half2 a = __hmax2(__habs2(lo), __habs2(hi));
+  float m = fmaxf(__low2float(a), __high2float(a));
+#pragma unroll
+  for (int o = D / 8; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(D == 128 ? 0xffffffffu : 0xffffu, m, o));
+  return m;
+}
+
+// E4M3 row store (common.cuh): thread j holds elements (2j, 2j+1) and (D/2 + 2j, D/2 + 2j + 1) of the row
+template <int D>
+__device__ __forceinline__ void store_row_e4m3(__half2 lo, __half2 hi, uint8_t* codes_row, int8_t* exp, int j) {
+  const int e = kv_e4m3_exponent(row_amax<D>(lo, hi));
+  const float2 l = __half22float2(lo), u = __half22float2(hi);
+  reinterpret_cast<uint16_t*>(codes_row)[j] = kv_e4m3_quantize2(l.x, l.y, e);
+  reinterpret_cast<uint16_t*>(codes_row)[j + D / 4] = kv_e4m3_quantize2(u.x, u.y, e);
+  if (j == 0) *exp = (int8_t)e;
+}
+
+// E4M3: Kc / Vc are the code stores [Hkv][cap][D] (head stride cap * D), Ke / Ve the exponents [Hkv][cap]
+template <int D, bool E4M3>
 __global__ void __launch_bounds__(D / 4) rope_append_kernel(const __half* __restrict__ q, const __half* __restrict__ k,
                                                             const __half* __restrict__ v, long long row_stride,
                                                             const __half* __restrict__ cos, const __half* __restrict__ sin,
@@ -22,8 +43,9 @@ __global__ void __launch_bounds__(D / 4) rope_append_kernel(const __half* __rest
                                                             const int32_t* __restrict__ pos0_dev, int slot0,
                                                             const int32_t* __restrict__ slot0_dev, int H, int Hkv, int rotate_q,
                                                             int rotate_k, __half* __restrict__ q_out,
-                                                            __half* __restrict__ Kc, __half* __restrict__ Vc,
-                                                            long long head_stride, long long cap) {
+                                                            void* __restrict__ Kc, void* __restrict__ Vc,
+                                                            long long head_stride, long long cap, int8_t* __restrict__ Ke,
+                                                            int8_t* __restrict__ Ve) {
   pdl_launch_dependents();
   pdl_wait();
   // one CTA per (row, query head); the first Hkv of them also append K/V head h (grouped-query attention: Hkv < H)
@@ -48,14 +70,47 @@ __global__ void __launch_bounds__(D / 4) rope_append_kernel(const __half* __rest
     const __half2* x = reinterpret_cast<const __half2*>(k + in);
     __half2 lo = x[j], hi = x[j + D / 4];
     if (rotate_k) rope_pair(lo, hi, cl, ch, sl, sh, lo, hi);
-    __half2* o = reinterpret_cast<__half2*>(Kc + dst);
-    o[j] = lo;
-    o[j + D / 4] = hi;
     const __half2* xv = reinterpret_cast<const __half2*>(v + in);
-    __half2* ov = reinterpret_cast<__half2*>(Vc + dst);
-    ov[j] = xv[j];
-    ov[j + D / 4] = xv[j + D / 4];
+    if constexpr (E4M3) {
+      const size_t ex = (size_t)h * cap + (size_t)slot;
+      store_row_e4m3<D>(lo, hi, reinterpret_cast<uint8_t*>(Kc) + dst, Ke + ex, j);
+      store_row_e4m3<D>(xv[j], xv[j + D / 4], reinterpret_cast<uint8_t*>(Vc) + dst, Ve + ex, j);
+    } else {
+      __half2* o = reinterpret_cast<__half2*>(reinterpret_cast<__half*>(Kc) + dst);
+      o[j] = lo;
+      o[j + D / 4] = hi;
+      __half2* ov = reinterpret_cast<__half2*>(reinterpret_cast<__half*>(Vc) + dst);
+      ov[j] = xv[j];
+      ov[j + D / 4] = xv[j + D / 4];
+    }
   }
+}
+
+// fp16 rows [slot0, slot0 + n) of one layer -> E4M3 codes and exponents, one warp per (row, KV head)
+template <int D>
+__global__ void __launch_bounds__(128) kv_quantize_kernel(const __half* __restrict__ src, long long src_head_stride, int slot0, int n,
+                                                          uint8_t* __restrict__ codes, int8_t* __restrict__ exps, long long cap) {
+  constexpr int EPL = D / 32;  // elements per lane
+  const int r = blockIdx.x * 4 + (threadIdx.x >> 5), h = blockIdx.y, lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const size_t slot = (size_t)slot0 + r;
+  const __half2* x = reinterpret_cast<const __half2*>(src + (size_t)h * src_head_stride + slot * D + lane * EPL);
+  __half2 v[EPL / 2];
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < EPL / 2; ++i) {
+    v[i] = x[i];
+    const __half2 a = __habs2(v[i]);
+    m = fmaxf(m, fmaxf(__low2float(a), __high2float(a)));
+  }
+  const int e = kv_e4m3_exponent(warp_max(m));
+  uint16_t* out = reinterpret_cast<uint16_t*>(codes + ((size_t)h * cap + slot) * D + lane * EPL);
+#pragma unroll
+  for (int i = 0; i < EPL / 2; ++i) {
+    const float2 f = __half22float2(v[i]);
+    out[i] = kv_e4m3_quantize2(f.x, f.y, e);
+  }
+  if (lane == 0) exps[(size_t)h * cap + slot] = (int8_t)e;
 }
 
 // ---- (ii) draft attention --------------------------------------------------------------------------------------------
@@ -191,6 +246,29 @@ __global__ void __launch_bounds__(256) tail_update_kernel(const __half* __restri
   }
 }
 
+// tail_update_kernel over an E4M3 store: codes and their exponents in, D out (exponent strides = code strides / D)
+__global__ void __launch_bounds__(256) tail_update_e4m3_kernel(const uint8_t* __restrict__ K, const uint8_t* __restrict__ V,
+                                                               const int8_t* __restrict__ Ke, const int8_t* __restrict__ Ve,
+                                                               long long kls, long long khs, __half* __restrict__ rK,
+                                                               __half* __restrict__ rV, long long rls, long long rhs, int D,
+                                                               int prefill, int budget, int seq_len_host,
+                                                               const int32_t* __restrict__ seq_len_dev) {
+  const int h = blockIdx.y, layer = blockIdx.z;
+  const int n_new = seq_len_host + (seq_len_dev ? *seq_len_dev : 0) - prefill;
+  if (n_new <= 0) return;
+  const int vec_per_row = D / 8;
+  const int total = n_new * vec_per_row;
+  const size_t head = (size_t)layer * kls + (size_t)h * khs;
+  const size_t dst0 = (size_t)layer * rls + (size_t)h * rhs + (size_t)(budget - n_new) * D;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const size_t slot = (size_t)prefill + i / vec_per_row;
+    const size_t src = head + slot * D + (size_t)(i % vec_per_row) * 8;
+    const size_t ex = head / D + slot;
+    *reinterpret_cast<uint4*>(rK + dst0 + (size_t)i * 8) = kv_e4m3_dequant8(*reinterpret_cast<const uint2*>(K + src), Ke[ex]);
+    *reinterpret_cast<uint4*>(rV + dst0 + (size_t)i * 8) = kv_e4m3_dequant8(*reinterpret_cast<const uint2*>(V + src), Ve[ex]);
+  }
+}
+
 __global__ void __launch_bounds__(256) window_slide_kernel(__half* __restrict__ K, __half* __restrict__ V, long long ls,
                                                            long long hs, int D, int src_start, int dst_start, int n_rows) {
   extern __shared__ __align__(16) uint8_t wsm[];
@@ -314,10 +392,13 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const __half* __restrict_
 extern "C" {
 
 // H query heads, Hkv K/V heads (Hkv == H: MHA)
+// Kexp / Vexp non-NULL: Kcache / Vcache are E4M3 code stores of one layer ([Hkv][cap][d], head stride cap * d) with these
+// exponents [Hkv][cap]
 static int rope_append_impl(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
                             int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
                             const int32_t* slot0_dev, int R, int H, int Hkv, int d, int rotate_q, int rotate_k, void* q_out,
-                            void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream_) {
+                            void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream_,
+                            int8_t* Kexp = nullptr, int8_t* Vexp = nullptr) {
   using namespace tf;
   TF_CHECK_ARG(q && k && v && cos && sin && q_out && Kcache && Vcache, "tf_rope_append: NULL pointer");
   TF_CHECK_ARG(R >= 1 && H >= 1 && max_pos >= 1 && cap >= 1, "tf_rope_append: bad extents");
@@ -327,16 +408,19 @@ static int rope_append_impl(const void* q, const void* k, const void* v, long lo
   if (!slot0_dev) TF_CHECK_ARG(slot0 >= 0 && (long long)slot0 + R <= cap, "tf_rope_append: slots [%d,%d) exceed capacity %lld", slot0, slot0 + R, cap);
   dim3 grid(R, H);
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (d == 128)
-    TF_CHECK_CUDA(launch_kernel(kPdlRope, rope_append_kernel<128>, grid, 32, 0, stream, (const __half*)q, (const __half*)k, (const __half*)v, qkv_row_stride,
-                                                     (const __half*)cos, (const __half*)sin, max_pos, pos_ids_dev, pos0, pos0_dev,
-                                                     slot0, slot0_dev, H, Hkv, rotate_q, rotate_k, (__half*)q_out, (__half*)Kcache,
-                                                     (__half*)Vcache, kv_head_stride, cap));
-  else
-    TF_CHECK_CUDA(launch_kernel(kPdlRope, rope_append_kernel<64>, grid, 16, 0, stream, (const __half*)q, (const __half*)k, (const __half*)v, qkv_row_stride,
-                                                    (const __half*)cos, (const __half*)sin, max_pos, pos_ids_dev, pos0, pos0_dev,
-                                                    slot0, slot0_dev, H, Hkv, rotate_q, rotate_k, (__half*)q_out, (__half*)Kcache,
-                                                    (__half*)Vcache, kv_head_stride, cap));
+#define TF_LAUNCH_ROPE(D_, E4M3_)                                                                                                   \
+  TF_CHECK_CUDA(launch_kernel(kPdlRope, rope_append_kernel<D_, E4M3_>, grid, D_ / 4, 0, stream, (const __half*)q, (const __half*)k,  \
+                              (const __half*)v, qkv_row_stride, (const __half*)cos, (const __half*)sin, max_pos, pos_ids_dev, pos0, \
+                              pos0_dev, slot0, slot0_dev, H, Hkv, rotate_q, rotate_k, (__half*)q_out, Kcache, Vcache,              \
+                              kv_head_stride, cap, Kexp, Vexp))
+  if (Kexp) {
+    if (d == 128) TF_LAUNCH_ROPE(128, true);
+    else TF_LAUNCH_ROPE(64, true);
+  } else {
+    if (d == 128) TF_LAUNCH_ROPE(128, false);
+    else TF_LAUNCH_ROPE(64, false);
+  }
+#undef TF_LAUNCH_ROPE
   TF_CHECK_LAUNCH();
   return TF_OK;
 }
@@ -355,6 +439,33 @@ int tf_rope_append_gqa(const void* q, const void* k, const void* v, long long qk
                        void* Kcache, void* Vcache, long long kv_head_stride, long long cap, tf_stream_t stream) {
   return rope_append_impl(q, k, v, qkv_row_stride, cos, sin, max_pos, pos_ids_dev, pos0, pos0_dev, slot0, slot0_dev, R, Hq, Hkv, d,
                           rotate_q, rotate_k, q_out, Kcache, Vcache, kv_head_stride, cap, stream);
+}
+
+int tf_rope_append_e4m3(const void* q, const void* k, const void* v, long long qkv_row_stride, const void* cos, const void* sin,
+                        int max_pos, const int32_t* pos_ids_dev, int pos0, const int32_t* pos0_dev, int slot0,
+                        const int32_t* slot0_dev, int R, int Hq, int Hkv, int d, void* q_out, void* Kcodes, void* Vcodes,
+                        int8_t* Kexp, int8_t* Vexp, long long cap, tf_stream_t stream) {
+  TF_CHECK_ARG(Kexp && Vexp, "tf_rope_append_e4m3: NULL exponent pointer");
+  return rope_append_impl(q, k, v, qkv_row_stride, cos, sin, max_pos, pos_ids_dev, pos0, pos0_dev, slot0, slot0_dev, R, Hq, Hkv, d,
+                          1, 1, q_out, Kcodes, Vcodes, cap * d, cap, stream, Kexp, Vexp);
+}
+
+int tf_kv_quantize_e4m3(const void* src, long long src_head_stride, int slot0, int n, int Hkv, int d, void* codes, int8_t* exps,
+                        long long cap, tf_stream_t stream_) {
+  using namespace tf;
+  TF_CHECK_ARG(src && codes && exps, "tf_kv_quantize_e4m3: NULL pointer");
+  TF_CHECK_SUPPORTED(d == 64 || d == 128, "tf_kv_quantize_e4m3: head_dim %d not in {64,128}", d);
+  TF_CHECK_ARG(Hkv >= 1 && n >= 0 && slot0 >= 0 && (long long)slot0 + n <= cap, "tf_kv_quantize_e4m3: rows [%d,%d) outside [0,%lld)",
+               slot0, slot0 + n, cap);
+  TF_CHECK_ARG(src_head_stride >= cap * d && src_head_stride % 8 == 0 && ((uintptr_t)src & 15) == 0 && ((uintptr_t)codes & 15) == 0,
+               "tf_kv_quantize_e4m3: src must be 16-byte aligned with a head stride of at least cap*d elements (a multiple of 8)");
+  if (n == 0) return TF_OK;
+  dim3 grid((n + 3) / 4, Hkv);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (d == 128) kv_quantize_kernel<128><<<grid, 128, 0, stream>>>((const __half*)src, src_head_stride, slot0, n, (uint8_t*)codes, exps, cap);
+  else kv_quantize_kernel<64><<<grid, 128, 0, stream>>>((const __half*)src, src_head_stride, slot0, n, (uint8_t*)codes, exps, cap);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
 }
 
 int tf_draft_attn(const void* q, const void* K, const void* V, long long kv_head_stride, const void* cos, const void* sin,
@@ -400,6 +511,32 @@ int tf_tail_update(const void* K, const void* V, long long kv_layer_stride, long
   tail_update_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>((const __half*)K, (const __half*)V, kv_layer_stride, kv_head_stride,
                                                               (__half*)retrK, (__half*)retrV, r_layer_stride, r_head_stride, d,
                                                               prefill, budget, seq_len_host, seq_len_dev);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_tail_update_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                        long long kv_head_stride, void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride,
+                        int n_layers, int H, int d, int prefill, int budget, int seq_len_host, const int32_t* seq_len_dev,
+                        int max_new, tf_stream_t stream_) {
+  using namespace tf;
+  TF_CHECK_ARG(K && V && Kexp && Vexp && retrK && retrV, "tf_tail_update_e4m3: NULL pointer");
+  TF_CHECK_ARG(n_layers >= 1 && H >= 1 && d % 8 == 0, "tf_tail_update_e4m3: bad extents");
+  TF_CHECK_ARG(kv_layer_stride % d == 0 && kv_head_stride % d == 0 && ((((uintptr_t)K | (uintptr_t)V)) & 7) == 0,
+               "tf_tail_update_e4m3: code strides must be multiples of d and codes 8-byte aligned");
+  TF_CHECK_ARG(max_new >= 0 && max_new <= budget, "tf_tail_update_e4m3: max_new %d exceeds budget %d", max_new, budget);
+  if (!seq_len_dev) {
+    TF_CHECK_ARG(seq_len_host - prefill <= budget, "tf_tail_update_e4m3: %d new tokens exceed budget %d", seq_len_host - prefill, budget);
+    if (seq_len_host <= prefill) return TF_OK;
+    max_new = seq_len_host - prefill;
+  }
+  if (max_new == 0) return TF_OK;
+  int gx = (max_new * (d / 8) + 255) / 256;
+  if (gx > 16) gx = 16;
+  dim3 grid(gx, H, n_layers);
+  tail_update_e4m3_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>((const uint8_t*)K, (const uint8_t*)V, Kexp, Vexp, kv_layer_stride,
+                                                                   kv_head_stride, (__half*)retrK, (__half*)retrV, r_layer_stride,
+                                                                   r_head_stride, d, prefill, budget, seq_len_host, seq_len_dev);
   TF_CHECK_LAUNCH();
   return TF_OK;
 }

@@ -6,6 +6,8 @@
 //   order  = descending score, ascending chunk index on ties, -0 == +0, NaN greatest; chunk 0 forced first.
 // Grouped-query attention (tf_retrieval_build_gqa, rule "group_sum"): scores, top-k and gather run per (layer, KV head) and
 // the score's query is q̄ = fp64 sum of the grp query heads of the group (exact for grp <= 64 fp16 values); grp = 1 is MHA.
+// E4M3 store (tf_retrieval_build_e4m3, the format of common.cuh): scores and gather read the codes and exponents, and every
+// K or V value they use is D, so results are those of the fp16 build on D; the gather writes D into the fp16 retrieval cache.
 // All three kernels are HBM/latency bound integer+fp work; no tensor cores (task statement ①).
 #include "common.cuh"
 
@@ -15,17 +17,25 @@ namespace tf {
 // kernel 1: scores.  One lane group (d/8 lanes) owns one chunk: every lane keeps an 8-wide slice of the running mean.
 // A warp therefore streams 32/(d/8) chunks at once; loads are 16-byte, fully coalesced (a row = d*2 contiguous bytes).
 // --------------------------------------------------------------------------------------------------------------------
-template <int D, int CHUNK /* 0 = runtime */>
-__global__ void __launch_bounds__(256) chunk_score_kernel(const __half* __restrict__ K, long long layer_stride,
+// 8 consecutive fp16 values of row `row` of a head, from the fp16 store or (Ke != NULL) as D of the E4M3 store
+template <bool E4M3>
+__device__ __forceinline__ uint4 load8(const void* base, size_t off, const int8_t* __restrict__ Ke, size_t row) {
+  if constexpr (E4M3) return kv_e4m3_dequant8(__ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(base) + off)), Ke[row]);
+  else return ld_nc_v4(reinterpret_cast<const __half*>(base) + off);
+}
+
+template <int D, int CHUNK /* 0 = runtime */, bool E4M3>
+__global__ void __launch_bounds__(256) chunk_score_kernel(const void* __restrict__ K, long long layer_stride,
                                                           long long head_stride, const __half* __restrict__ q,
-                                                          int H, int qg, int chunks, int chunk_rt, __half* __restrict__ scores) {
+                                                          int H, int qg, int chunks, int chunk_rt, __half* __restrict__ scores,
+                                                          const int8_t* __restrict__ Ke) {
   constexpr int LPR = D / 8;        // lanes per row
   constexpr int CPW = 32 / LPR;     // chunks per warp pass
   const int chunk = CHUNK ? CHUNK : chunk_rt;
   const int h = blockIdx.y, layer = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int grp = lane / LPR, li = lane % LPR;
-  const __half* Kh = K + (size_t)layer * layer_stride + (size_t)h * head_stride;
+  const size_t head0 = (size_t)layer * layer_stride + (size_t)h * head_stride;  // elements (fp16) or bytes (codes)
   const __half* qh = q + ((size_t)layer * H + h) * qg * D + li * 8;  // the qg query heads of KV head h
   double q64[8];
 #pragma unroll
@@ -46,11 +56,12 @@ __global__ void __launch_bounds__(256) chunk_score_kernel(const __half* __restri
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc[i] = 0.f;
     if (valid) {
-      const __half* base = Kh + (size_t)c * chunk * D + li * 8;
+      const size_t base = head0 + (size_t)c * chunk * D + li * 8;
+      const size_t row0 = head0 / D + (size_t)c * chunk;
       if (CHUNK == 8) {
         uint4 raw[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) raw[j] = ld_nc_v4(base + (size_t)j * D);  // 8 independent 16 B loads in flight
+        for (int j = 0; j < 8; ++j) raw[j] = load8<E4M3>(K, base + (size_t)j * D, Ke, row0 + j);  // 8 independent loads in flight
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const __half2* h2 = reinterpret_cast<const __half2*>(&raw[j]);
@@ -63,7 +74,7 @@ __global__ void __launch_bounds__(256) chunk_score_kernel(const __half* __restri
         }
       } else {
         for (int j = 0; j < chunk; ++j) {
-          uint4 raw = ld_nc_v4(base + (size_t)j * D);
+          uint4 raw = load8<E4M3>(K, base + (size_t)j * D, Ke, row0 + j);
           const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
@@ -172,12 +183,14 @@ __global__ void __launch_bounds__(1024) topk_kernel(const __half* __restrict__ s
 // kernel 3: gather.  In the head-major layout one chunk of one head is `chunk*d*2` contiguous bytes in both source and
 // destination, so the gather is a batch of small contiguous copies (16 B per thread).
 // --------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) gather_kernel(const __half* __restrict__ K, const __half* __restrict__ V,
+template <bool E4M3>
+__global__ void __launch_bounds__(256) gather_kernel(const void* __restrict__ K, const void* __restrict__ V,
                                                      long long kv_layer_stride, long long kv_head_stride,
                                                      __half* __restrict__ rK, __half* __restrict__ rV,
                                                      long long r_layer_stride, long long r_head_stride,
                                                      const int32_t* __restrict__ idx, int H, int select_sets,
-                                                     int chunk_elems /* chunk*d */) {
+                                                     int chunk_elems /* chunk*d */, int d, const int8_t* __restrict__ Ke,
+                                                     const int8_t* __restrict__ Ve) {
   const int h = blockIdx.y, layer = blockIdx.z;
   const int vec_per_chunk = chunk_elems / 8;
   const size_t row = (size_t)layer * H + h;
@@ -189,8 +202,9 @@ __global__ void __launch_bounds__(256) gather_kernel(const __half* __restrict__ 
     const int slot = i / vec_per_chunk, v = i % vec_per_chunk;
     const size_t src = src_base + (size_t)id[slot] * chunk_elems + (size_t)v * 8;
     const size_t dst = dst_base + (size_t)slot * chunk_elems + (size_t)v * 8;
-    const uint4 a = ld_nc_v4(K + src);
-    const uint4 b = ld_nc_v4(V + src);
+    const size_t src_row = src / d;  // exponent index of the source row
+    const uint4 a = load8<E4M3>(K, src, Ke, src_row);
+    const uint4 b = load8<E4M3>(V, src, Ve, src_row);
     *reinterpret_cast<uint4*>(rK + dst) = a;
     *reinterpret_cast<uint4*>(rV + dst) = b;
   }
@@ -207,10 +221,12 @@ static int next_pow2(int x) {
 extern "C" {
 
 // H = KV heads of the store; the query has H * grp heads (grp = 1: MHA)
+// Ke / Ve non-NULL: K / V are E4M3 code stores with these exponents (strides in bytes; exponent strides = code strides / d)
 static int retrieval_build_impl(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
                                 int n_layers, int H, int grp, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
                                 long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
-                                void* workspace, size_t workspace_bytes, tf_stream_t stream_);
+                                void* workspace, size_t workspace_bytes, tf_stream_t stream_, const int8_t* Ke = nullptr,
+                                const int8_t* Ve = nullptr);
 
 size_t tf_retrieval_build_workspace_bytes(int n_layers, int H, int d, int prefill, int chunk, int budget) {
   if (n_layers <= 0 || H <= 0 || chunk <= 0) return 0;
@@ -225,6 +241,26 @@ int tf_retrieval_build(const void* K, const void* V, long long kv_layer_stride, 
                        void* workspace, size_t workspace_bytes, tf_stream_t stream) {
   return retrieval_build_impl(K, V, kv_layer_stride, kv_head_stride, q, n_layers, H, 1, d, prefill, chunk, budget, retrK, retrV,
                               r_layer_stride, r_head_stride, out_idx, out_scores, workspace, workspace_bytes, stream);
+}
+
+int tf_retrieval_build_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                            long long kv_head_stride, const void* q, int n_layers, int Hq, int Hkv, int d, int prefill, int chunk,
+                            int budget, void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride, int32_t* out_idx,
+                            void* out_scores, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0 || Hq / Hkv > 64) {
+    tf::set_error("tf_retrieval_build_e4m3: Hq (%d) must be a multiple of Hkv (%d), at most 64 per KV head", Hq, Hkv);
+    return TF_ERR_INVALID;
+  }
+  if (!Kexp || !Vexp) {
+    tf::set_error("tf_retrieval_build_e4m3: NULL exponent pointer");
+    return TF_ERR_INVALID;
+  }
+  if (d <= 0 || kv_layer_stride % d != 0 || kv_head_stride % d != 0) {
+    tf::set_error("tf_retrieval_build_e4m3: code strides must be multiples of d");
+    return TF_ERR_INVALID;
+  }
+  return retrieval_build_impl(K, V, kv_layer_stride, kv_head_stride, q, n_layers, Hkv, Hq / Hkv, d, prefill, chunk, budget, retrK,
+                              retrV, r_layer_stride, r_head_stride, out_idx, out_scores, workspace, workspace_bytes, stream, Kexp, Vexp);
 }
 
 int tf_retrieval_build_gqa(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
@@ -242,14 +278,16 @@ int tf_retrieval_build_gqa(const void* K, const void* V, long long kv_layer_stri
 static int retrieval_build_impl(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
                                 int n_layers, int H, int grp, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
                                 long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
-                                void* workspace, size_t workspace_bytes, tf_stream_t stream_) {
+                                void* workspace, size_t workspace_bytes, tf_stream_t stream_, const int8_t* Ke, const int8_t* Ve) {
   using namespace tf;
+  const bool e4m3 = Ke != nullptr;
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(K && V && q && retrK && retrV, "tf_retrieval_build: NULL pointer");
   TF_CHECK_ARG(n_layers > 0 && H > 0 && chunk > 0, "tf_retrieval_build: bad extents");
   TF_CHECK_ARG(prefill % chunk == 0, "prefill should be multiple of chunk_size, got %d %% %d", prefill, chunk);
   TF_CHECK_ARG(budget % chunk == 0, "max_budget should be multiple of chunk_size, got %d %% %d", budget, chunk);
   TF_CHECK_SUPPORTED(d == 64 || d == 128 || d == 256, "tf_retrieval_build: head_dim %d not in {64,128,256}", d);
+  TF_CHECK_SUPPORTED(!e4m3 || d != 256, "tf_retrieval_build_e4m3: head_dim %d not in {64,128}", d);
   const int chunks = prefill / chunk, sel = budget / chunk;
   TF_CHECK_ARG(sel >= 1 && sel - 1 <= chunks - 1, "selected index k out of range (k=%d, candidates=%d)", sel - 1, chunks - 1);
   TF_CHECK_ARG(((uintptr_t)K & 15) == 0 && ((uintptr_t)V & 15) == 0 && ((uintptr_t)retrK & 15) == 0 &&
@@ -281,12 +319,15 @@ static int retrieval_build_impl(const void* K, const void* V, long long kv_layer
     const int cap = (sms * 8 + H * n_layers - 1) / (H * n_layers);
     if (gx > cap) gx = cap < 1 ? 1 : cap;
     dim3 grid(gx, H, n_layers);
-#define LAUNCH_SCORE(D_, C_)                                                                                        \
-  chunk_score_kernel<D_, C_><<<grid, 256, 0, stream>>>((const __half*)K, kv_layer_stride, kv_head_stride,          \
-                                                       (const __half*)q, H, grp, chunks, chunk, scores)
-    if (d == 128) { if (chunk == 8) LAUNCH_SCORE(128, 8); else LAUNCH_SCORE(128, 0); }
-    else if (d == 64) { if (chunk == 8) LAUNCH_SCORE(64, 8); else LAUNCH_SCORE(64, 0); }
-    else { if (chunk == 8) LAUNCH_SCORE(256, 8); else LAUNCH_SCORE(256, 0); }
+#define LAUNCH_SCORE(D_, C_, E_)                                                                                    \
+  chunk_score_kernel<D_, C_, E_><<<grid, 256, 0, stream>>>(K, kv_layer_stride, kv_head_stride, (const __half*)q, H, grp, \
+                                                           chunks, chunk, scores, Ke)
+    if (e4m3) {
+      if (d == 128) { if (chunk == 8) LAUNCH_SCORE(128, 8, true); else LAUNCH_SCORE(128, 0, true); }
+      else { if (chunk == 8) LAUNCH_SCORE(64, 8, true); else LAUNCH_SCORE(64, 0, true); }
+    } else if (d == 128) { if (chunk == 8) LAUNCH_SCORE(128, 8, false); else LAUNCH_SCORE(128, 0, false); }
+    else if (d == 64) { if (chunk == 8) LAUNCH_SCORE(64, 8, false); else LAUNCH_SCORE(64, 0, false); }
+    else { if (chunk == 8) LAUNCH_SCORE(256, 8, false); else LAUNCH_SCORE(256, 0, false); }
 #undef LAUNCH_SCORE
     TF_CHECK_LAUNCH();
   }
@@ -300,9 +341,12 @@ static int retrieval_build_impl(const void* K, const void* V, long long kv_layer
     int gx = (total_vec + 255) / 256;
     if (gx > 64) gx = 64;
     dim3 grid(gx, H, n_layers);
-    gather_kernel<<<grid, 256, 0, stream>>>((const __half*)K, (const __half*)V, kv_layer_stride, kv_head_stride,
-                                            (__half*)retrK, (__half*)retrV, r_layer_stride, r_head_stride, idx, H, sel,
-                                            chunk * d);
+    if (e4m3)
+      gather_kernel<true><<<grid, 256, 0, stream>>>(K, V, kv_layer_stride, kv_head_stride, (__half*)retrK, (__half*)retrV,
+                                                    r_layer_stride, r_head_stride, idx, H, sel, chunk * d, d, Ke, Ve);
+    else
+      gather_kernel<false><<<grid, 256, 0, stream>>>(K, V, kv_layer_stride, kv_head_stride, (__half*)retrK, (__half*)retrV,
+                                                     r_layer_stride, r_head_stride, idx, H, sel, chunk * d, d, nullptr, nullptr);
     TF_CHECK_LAUNCH();
   }
   return TF_OK;

@@ -18,6 +18,9 @@
 //     head h reads KV head h / grp): the work units are (KV head, tile) and a CTA computes the R * grp packed rows of
 //     all query heads of a group against every tile it loads, so each K/V byte is still read once per launch.
 //     "Head" below means KV head; MHA is grp = 1 and runs the same code.
+//   * an E4M3 store (tf_verify_attn_e4m3, the format of common.cuh): the same kernel with KV = __nv_fp8_e4m3.  A stage carries
+//     the 64-key code tiles (TMA) and the tiles' 64 + 64 exponents (bulk copy); twice the stages keep the fp16 ring's bytes in
+//     flight.  No calibrated split, L2 prefetch or tree mode.
 //   * the split is equal by default.  SMs need not all pull the same HBM bandwidth (GPC-level sharing; per-CTA
 //     %globaltimer stamps show it, tools/attn_timing.py), so under an equal split the kernel waits on the slowest GPCs.
 //     tf_verify_attn_calibrate
@@ -32,6 +35,8 @@
 
 #include <algorithm>
 #include <vector>
+
+#include <cuda_fp8.h>
 
 #include "common.cuh"
 
@@ -99,23 +104,53 @@ __device__ __forceinline__ unsigned long long global_ns() {
 constexpr int kSplitHdr = 4;  // u32 header words of a split table: {G the table was calibrated for, 0, 0, 0}
 
 struct AttnSmemLayout {
-  // dynamic shared memory: [STAGES][K tile | V tile] (1024-aligned) | Osh | msh | lsh | barriers
-  static __host__ __device__ size_t tile_bytes(int D) { return (size_t)BN * D * 2; }
-  static __host__ __device__ size_t bytes(int D, int MT, int stages) {
-    return 1024 /*align slack*/ + (size_t)stages * 2 * tile_bytes(D) + (size_t)16 * MT * D * 4 + 2 * 4 * 32 * 4 + 2 * 8 * stages + 64;
+  // dynamic shared memory: [STAGES][K tile | V tile] (1024-aligned) | e4m3 only: [STAGES][K exponents | V exponents] |
+  // Osh | msh | lsh | barriers
+  static __host__ __device__ size_t tile_bytes(int D, int eb) { return (size_t)BN * D * eb; }
+  static __host__ __device__ size_t exp_bytes(int eb) { return eb == 1 ? (size_t)2 * BN : 0; }
+  static __host__ __device__ size_t bytes(int D, int MT, int stages, int eb) {
+    return 1024 /*align slack*/ + (size_t)stages * (2 * tile_bytes(D, eb) + exp_bytes(eb)) + (size_t)16 * MT * D * 4 + 2 * 4 * 32 * 4 +
+           2 * 8 * stages + 64;
   }
 };
 
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
+  uint32_t r;
+  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
+  return r;
+}
+__device__ __forceinline__ uint32_t h2u(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+// 1-D bulk copy global -> shared completing on an mbarrier (16-byte aligned, size % 16 == 0)
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(smem_dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+
 constexpr int kPfChunk = 4096;  // bytes per L2 prefetch request (tf_verify_attn_prefetch)
 
-template <int D, int MT, int STAGES>
+// KV = __half: the fp16 store.  KV = __nv_fp8_e4m3: the E4M3 store of common.cuh, codes through kmap / vmap and exponents
+// [layer][H][cap] in k_exp / v_exp.  sm_90 has no 8-bit ldmatrix, so the e4m3 fragments are built from 32-bit shared loads:
+//   K: a thread's word holds d elements 4tq..4tq+3 of one key and stands for the mma's k positions {2tq, 2tq+1, 2tq+8, 2tq+9};
+//      the Q fragment is loaded in the same order, so the dot product is unchanged.  K exponents scale the score columns:
+//      (q·code)·2^e equals q·D unless D itself rounds (e < -15, or a ±65504 row whose D is ±inf; see the header).
+//   V: words of key rows (k, k+1) are interleaved byte-wise (prmt) into e4m3 pairs along the mma's k axis; a thread's word holds
+//      4 d columns, so n-block 4j+i carries columns 32j + 4n + i at mma column n, and O is written back in that order.  V is
+//      dequantized exactly to D (kv_e4m3_apply) before the PV mma.
+template <typename KV, int D, int MT, int STAGES>
 __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_mma_kernel(
     const __grid_constant__ CUtensorMap kmap, const __grid_constant__ CUtensorMap vmap, const __half* __restrict__ q,
     int layer, int kv_len_host, const int32_t* __restrict__ kv_len_dev, int R, int H, int grp, float scale_log2,
     float* __restrict__ part_m, float* __restrict__ part_l, float* __restrict__ part_o, int* __restrict__ head_counters,
     __half* __restrict__ out, const uint32_t* __restrict__ tree_mask, int tree_cols,
     const uint32_t* __restrict__ split_table, uint32_t* __restrict__ cta_ns, int clean_keys, const uint8_t* __restrict__ pf_ptr,
-    uint32_t pf_chunks) {
+    uint32_t pf_chunks, const int8_t* __restrict__ k_exp, const int8_t* __restrict__ v_exp, long long cap) {
+  constexpr bool kE4m3 = sizeof(KV) == 1;
   constexpr int NKW = kConsumerWarps / MT;  // warps along the key axis
   constexpr int KW = BN / NKW;              // keys per warp per tile (16 or 32)
   constexpr int NB = KW / 8;                // score n-blocks per warp
@@ -123,13 +158,16 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
   constexpr int DK = D / 16;                // QK k-steps
   constexpr int DN = D / 8;                 // output n-blocks
   constexpr int SUBS = D / 64;              // 64-element (128 B) swizzle spans per row
-  constexpr uint32_t TILE_BYTES = BN * D * 2;
+  constexpr uint32_t TILE_BYTES = BN * D * sizeof(KV);
   constexpr uint32_t SUB_BYTES = BN * 128;
+  constexpr uint32_t EXP_BYTES = kE4m3 ? 2 * BN : 0;  // per stage: K then V exponents of the tile's keys
+  constexpr uint32_t ROW_BYTES = D * sizeof(KV);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* tiles = smem;
-  float* Osh = reinterpret_cast<float*>(tiles + (size_t)STAGES * 2 * TILE_BYTES);  // [16*MT][D]
+  int8_t* exps = reinterpret_cast<int8_t*>(tiles + (size_t)STAGES * 2 * TILE_BYTES);
+  float* Osh = reinterpret_cast<float*>(tiles + (size_t)STAGES * (2 * TILE_BYTES + EXP_BYTES));  // [16*MT][D]
   float* msh = Osh + 16 * MT * D;                                                 // [NKW][16*MT]  (<= 4*32)
   float* lsh = msh + 4 * 32;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(lsh + 4 * 32);
@@ -184,13 +222,21 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       auto issue = [&](uint32_t gt_, uint32_t s) {
         const int h = (int)(gt_ / tph);
         const int key0 = (int)(gt_ % tph) * BN;
-        mbar_expect_tx(&full_bar[s], 2 * TILE_BYTES);
+        mbar_expect_tx(&full_bar[s], 2 * TILE_BYTES + EXP_BYTES);
         uint8_t* kt = tiles + (size_t)s * 2 * TILE_BYTES;
         uint8_t* vt = kt + TILE_BYTES;
+        if constexpr (kE4m3) {
+          tma_load_4d(kt, &kmap, &full_bar[s], 0, key0, h, layer);
+          tma_load_4d(vt, &vmap, &full_bar[s], 0, key0, h, layer);
+          const size_t e0 = ((size_t)layer * H + h) * (size_t)cap + key0;
+          bulk_load(exps + (size_t)s * EXP_BYTES, k_exp + e0, BN, &full_bar[s]);
+          bulk_load(exps + (size_t)s * EXP_BYTES + BN, v_exp + e0, BN, &full_bar[s]);
+        } else {
 #pragma unroll
-        for (int sub = 0; sub < SUBS; ++sub) {
-          tma_load_4d(kt + sub * SUB_BYTES, &kmap, &full_bar[s], sub * 64, key0, h, layer);
-          tma_load_4d(vt + sub * SUB_BYTES, &vmap, &full_bar[s], sub * 64, key0, h, layer);
+          for (int sub = 0; sub < SUBS; ++sub) {
+            tma_load_4d(kt + sub * SUB_BYTES, &kmap, &full_bar[s], sub * 64, key0, h, layer);
+            tma_load_4d(vt + sub * SUB_BYTES, &vmap, &full_bar[s], sub * 64, key0, h, layer);
+          }
         }
       };
       // L2 prefetch of the weights the NEXT kernel streams (o_proj after a short-store attention, which is latency-bound and
@@ -213,18 +259,9 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
         pdl_wait();
       }
       for (; gt < end; ++gt, ++it) {
-        const int h = (int)(gt / tph);
-        const int key0 = (int)(gt % tph) * BN;
         const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
         mbar_wait(&empty_bar[s], ph ^ 1u);
-        mbar_expect_tx(&full_bar[s], 2 * TILE_BYTES);
-        uint8_t* kt = tiles + (size_t)s * 2 * TILE_BYTES;
-        uint8_t* vt = kt + TILE_BYTES;
-#pragma unroll
-        for (int sub = 0; sub < SUBS; ++sub) {
-          tma_load_4d(kt + sub * SUB_BYTES, &kmap, &full_bar[s], sub * 64, key0, h, layer);
-          tma_load_4d(vt + sub * SUB_BYTES, &vmap, &full_bar[s], sub * 64, key0, h, layer);
-        }
+        issue(gt, s);
         pf_step();
       }
     }
@@ -255,11 +292,13 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       const __half* q1 = q + ((size_t)tr1 * Hq + h * grp + row1 % grp) * D;
 #pragma unroll
       for (int kk = 0; kk < DK; ++kk) {
-        const int c = kk * 16 + 2 * tq;
+        // mma k positions (2tq, 2tq+1 | 2tq+8, 2tq+9) hold d (c, c+1 | c2, c2+1): in order, or as the e4m3 K word lays them out
+        const int c = kk * 16 + (kE4m3 ? 4 * tq : 2 * tq);
+        const int c2 = kE4m3 ? c + 2 : c + 8;
         qa[kk][0] = row0 < rows ? *reinterpret_cast<const uint32_t*>(q0 + c) : 0u;
         qa[kk][1] = row1 < rows ? *reinterpret_cast<const uint32_t*>(q1 + c) : 0u;
-        qa[kk][2] = row0 < rows ? *reinterpret_cast<const uint32_t*>(q0 + c + 8) : 0u;
-        qa[kk][3] = row1 < rows ? *reinterpret_cast<const uint32_t*>(q1 + c + 8) : 0u;
+        qa[kk][2] = row0 < rows ? *reinterpret_cast<const uint32_t*>(q0 + c2) : 0u;
+        qa[kk][3] = row1 < rows ? *reinterpret_cast<const uint32_t*>(q1 + c2) : 0u;
       }
     }
     // ---- which CTAs deliver partials of head h: the owners of its first and last tile ----
@@ -285,6 +324,12 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       if (it == 0) TF_STAMP(1);
       const uint32_t kt = smem_u32(tiles + (size_t)s * 2 * TILE_BYTES);
       const uint32_t vt = kt + TILE_BYTES;
+      const int8_t* kx = exps + (size_t)s * EXP_BYTES;  // e4m3: exponents of the tile's keys
+      const int8_t* vx = kx + BN;
+      // byte offset of 16-byte chunk `chunk` of e4m3 key row `row` (SWIZZLE_128B rows of 128 B, SWIZZLE_64B rows of 64 B)
+      auto e4m3_chunk = [&](int row, int chunk) -> uint32_t {
+        return (uint32_t)(row * ROW_BYTES + ((chunk ^ (D == 128 ? (row & 7) : ((row >> 1) & 3))) << 4));
+      };
 
       // ---- S = Q K^T for this warp's KW keys ----
       float sc[NB][4];
@@ -292,16 +337,33 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       for (int n = 0; n < NB; ++n) { sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f; }
 #pragma unroll
       for (int kk = 0; kk < DK; ++kk) {
+        if constexpr (kE4m3) {
 #pragma unroll
-        for (int np = 0; np < NB / 2; ++np) {
-          const int mat = lane >> 3;
-          const int krow = kbase + (np * 2 + (mat >> 1)) * 8 + (lane & 7);
-          const int chunk = 2 * kk + (mat & 1);
-          const uint32_t addr = kt + (chunk >> 3) * SUB_BYTES + krow * 128 + (((chunk & 7) ^ (krow & 7)) << 4);
-          uint32_t b0, b1, b2, b3;
-          ldmatrix_x4(b0, b1, b2, b3, addr);
-          mma_16816(sc[np * 2], qa[kk], b0, b1);
-          mma_16816(sc[np * 2 + 1], qa[kk], b2, b3);
+          for (int n = 0; n < NB; ++n) {
+            const uint32_t w = lds32(kt + e4m3_chunk(kbase + n * 8 + g, kk) + 4 * tq);
+            mma_16816(sc[n], qa[kk], h2u(kv_e4m3_codes2((uint16_t)(w & 0xffffu))), h2u(kv_e4m3_codes2((uint16_t)(w >> 16))));
+          }
+        } else {
+#pragma unroll
+          for (int np = 0; np < NB / 2; ++np) {
+            const int mat = lane >> 3;
+            const int krow = kbase + (np * 2 + (mat >> 1)) * 8 + (lane & 7);
+            const int chunk = 2 * kk + (mat & 1);
+            const uint32_t addr = kt + (chunk >> 3) * SUB_BYTES + krow * 128 + (((chunk & 7) ^ (krow & 7)) << 4);
+            uint32_t b0, b1, b2, b3;
+            ldmatrix_x4(b0, b1, b2, b3, addr);
+            mma_16816(sc[np * 2], qa[kk], b0, b1);
+            mma_16816(sc[np * 2 + 1], qa[kk], b2, b3);
+          }
+        }
+      }
+      if constexpr (kE4m3) {  // score column j = (q . code_j) * 2^e_j
+#pragma unroll
+        for (int n = 0; n < NB; ++n) {
+          const int j = kbase + n * 8 + 2 * tq;
+          const float s0 = kv_e4m3_pow2(kx[j]), s1 = kv_e4m3_pow2(kx[j + 1]);
+          sc[n][0] *= s0; sc[n][2] *= s0;
+          sc[n][1] *= s1; sc[n][3] *= s1;
         }
       }
 
@@ -386,16 +448,42 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
       // ---- O += P V ----
 #pragma unroll
       for (int ks = 0; ks < KS; ++ks) {
+        if constexpr (kE4m3) {
+          // b0 = keys (k, k+1), b1 = keys (k+8, k+9) of column 32j + 4g + i, scaled per key to D
+          const int k = kbase + ks * 16 + 2 * tq;
+          __half a0, a1, a8, a9, m0_, m1_, m8_, m9_;
+          kv_e4m3_factors(vx[k], a0, m0_);
+          kv_e4m3_factors(vx[k + 1], a1, m1_);
+          kv_e4m3_factors(vx[k + 8], a8, m8_);
+          kv_e4m3_factors(vx[k + 9], a9, m9_);
+          const __half2 fa0 = __halves2half2(a0, a1), fb0 = __halves2half2(m0_, m1_);
+          const __half2 fa1 = __halves2half2(a8, a9), fb1 = __halves2half2(m8_, m9_);
 #pragma unroll
-        for (int nd = 0; nd < DN; nd += 2) {
-          const int mat = lane >> 3;
-          const int krow = kbase + ks * 16 + (mat & 1) * 8 + (lane & 7);
-          const int chunk = nd + (mat >> 1);
-          const uint32_t addr = vt + (chunk >> 3) * SUB_BYTES + krow * 128 + (((chunk & 7) ^ (krow & 7)) << 4);
-          uint32_t b0, b1, b2, b3;
-          ldmatrix_x4_trans(b0, b1, b2, b3, addr);
-          mma_16816(o[nd], pa[ks], b0, b1);
-          mma_16816(o[nd + 1], pa[ks], b2, b3);
+          for (int j = 0; j < DN / 4; ++j) {
+            const int chunk = 2 * j + (g >> 2), off = (g & 3) * 4;
+            const uint32_t w0 = lds32(vt + e4m3_chunk(k, chunk) + off), w1 = lds32(vt + e4m3_chunk(k + 1, chunk) + off);
+            const uint32_t w8 = lds32(vt + e4m3_chunk(k + 8, chunk) + off), w9 = lds32(vt + e4m3_chunk(k + 9, chunk) + off);
+            const uint32_t lo01 = prmt(w0, w1, 0x5140), hi01 = prmt(w0, w1, 0x7362);
+            const uint32_t lo89 = prmt(w8, w9, 0x5140), hi89 = prmt(w8, w9, 0x7362);
+            const uint32_t p0[4] = {lo01 & 0xffffu, lo01 >> 16, hi01 & 0xffffu, hi01 >> 16};
+            const uint32_t p8[4] = {lo89 & 0xffffu, lo89 >> 16, hi89 & 0xffffu, hi89 >> 16};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+              mma_16816(o[4 * j + i], pa[ks], h2u(kv_e4m3_apply(kv_e4m3_codes2((uint16_t)p0[i]), fa0, fb0)),
+                        h2u(kv_e4m3_apply(kv_e4m3_codes2((uint16_t)p8[i]), fa1, fb1)));
+          }
+        } else {
+#pragma unroll
+          for (int nd = 0; nd < DN; nd += 2) {
+            const int mat = lane >> 3;
+            const int krow = kbase + ks * 16 + (mat & 1) * 8 + (lane & 7);
+            const int chunk = nd + (mat >> 1);
+            const uint32_t addr = vt + (chunk >> 3) * SUB_BYTES + krow * 128 + (((chunk & 7) ^ (krow & 7)) << 4);
+            uint32_t b0, b1, b2, b3;
+            ldmatrix_x4_trans(b0, b1, b2, b3, addr);
+            mma_16816(o[nd], pa[ks], b0, b1);
+            mma_16816(o[nd + 1], pa[ks], b2, b3);
+          }
         }
       }
       __syncwarp();
@@ -432,16 +520,27 @@ __global__ void __launch_bounds__(kThreadsAttn, (MT == 1 ? 2 : 1)) verify_attn_m
         if (kslice == w) {
 #pragma unroll
           for (int n = 0; n < DN; ++n) {
-            const int c = n * 8 + 2 * tq;
-            float2* p0 = reinterpret_cast<float2*>(&Osh[row0 * D + c]);
-            float2* p1 = reinterpret_cast<float2*>(&Osh[row1 * D + c]);
-            float2 v0 = make_float2(o[n][0] * a0, o[n][1] * a0), v1 = make_float2(o[n][2] * a1, o[n][3] * a1);
-            if (w > 0) {
-              const float2 u0 = *p0, u1 = *p1;
-              v0.x += u0.x; v0.y += u0.y; v1.x += u1.x; v1.y += u1.y;
+            if constexpr (kE4m3) {  // mma columns (2tq, 2tq+1) of n-block n are d columns c and c + 4
+              const int c = 32 * (n >> 2) + 8 * tq + (n & 3);
+              float* p0 = Osh + row0 * D + c;
+              float* p1 = Osh + row1 * D + c;
+              const float v00 = o[n][0] * a0, v01 = o[n][1] * a0, v10 = o[n][2] * a1, v11 = o[n][3] * a1;
+              p0[0] = w > 0 ? p0[0] + v00 : v00;
+              p0[4] = w > 0 ? p0[4] + v01 : v01;
+              p1[0] = w > 0 ? p1[0] + v10 : v10;
+              p1[4] = w > 0 ? p1[4] + v11 : v11;
+            } else {
+              const int c = n * 8 + 2 * tq;
+              float2* p0 = reinterpret_cast<float2*>(&Osh[row0 * D + c]);
+              float2* p1 = reinterpret_cast<float2*>(&Osh[row1 * D + c]);
+              float2 v0 = make_float2(o[n][0] * a0, o[n][1] * a0), v1 = make_float2(o[n][2] * a1, o[n][3] * a1);
+              if (w > 0) {
+                const float2 u0 = *p0, u1 = *p1;
+                v0.x += u0.x; v0.y += u0.y; v1.x += u1.x; v1.y += u1.y;
+              }
+              *p0 = v0;
+              *p1 = v1;
             }
-            *p0 = v0;
-            *p1 = v1;
           }
         }
         named_bar_sync(1, kConsumerWarps * 32);
@@ -566,13 +665,14 @@ static int g_max_slots() {
   return sms * 2;
 }
 
-template <int D, int MT, int STAGES>
+template <typename KV, int D, int MT, int STAGES>
 static int launch_mma(const CUtensorMap& kmap, const CUtensorMap& vmap, const __half* q, int layer, int kv_len_host,
                       const int32_t* kv_len_dev, int R, int H, int grp, float scale_log2, float* pm, float* pl, float* po, int* counters,
                       __half* out, int G, const uint32_t* tree_mask, int tree_cols, const uint32_t* split_table, uint32_t* cta_ns,
-                      int clean_keys, bool allow_pdl, cudaStream_t stream, const uint8_t* pf_ptr, uint32_t pf_chunks) {
-  auto kern = verify_attn_mma_kernel<D, MT, STAGES>;
-  const size_t smem = AttnSmemLayout::bytes(D, MT, STAGES);
+                      int clean_keys, bool allow_pdl, cudaStream_t stream, const uint8_t* pf_ptr, uint32_t pf_chunks,
+                      const int8_t* k_exp, const int8_t* v_exp, long long cap) {
+  auto kern = verify_attn_mma_kernel<KV, D, MT, STAGES>;
+  const size_t smem = AttnSmemLayout::bytes(D, MT, STAGES, (int)sizeof(KV));
   int dev = 0;
   TF_CHECK_CUDA(cudaGetDevice(&dev));
   static bool attr_done[64] = {false};  // the attribute is per (function, device)
@@ -588,7 +688,7 @@ static int launch_mma(const CUtensorMap& kmap, const CUtensorMap& vmap, const __
   // block placement of a launch onto an EMPTY GPU — an early launch next to a draining predecessor changes it, which
   // can cost more than the overlap gains.  They still trigger their own dependents early.
   TF_CHECK_CUDA(launch_kernel(allow_pdl ? kPdlVerifyAttn : 0, kern, G, kThreadsAttn, smem, stream, kmap, vmap, q, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, pm, pl, po, counters,
-                              out, tree_mask, tree_cols, split_table, cta_ns, clean_keys, pf_ptr, pf_chunks));
+                              out, tree_mask, tree_cols, split_table, cta_ns, clean_keys, pf_ptr, pf_chunks, k_exp, v_exp, cap));
   TF_CHECK_LAUNCH();
   return TF_OK;
 }
@@ -672,7 +772,8 @@ static int verify_attn_impl(const void* q, const void* k_tensormap, const void* 
                             const int32_t* kv_len_dev, int kv_len_max, int R, int H, int grp, int d, float scale, void* out,
                             void* workspace, size_t workspace_bytes, int variant, const uint32_t* tree_mask, int tree_cols,
                             bool record_cta_ns, int clean_keys, tf_stream_t stream_, const void* next_weights = nullptr,
-                            size_t next_weight_bytes = 0) {
+                            size_t next_weight_bytes = 0, const int8_t* k_exp = nullptr, const int8_t* v_exp = nullptr,
+                            long long cap = 0) {
   using namespace tf;
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(q && k_tensormap && v_tensormap && out && workspace, "tf_verify_attn: NULL pointer");
@@ -695,7 +796,8 @@ static int verify_attn_impl(const void* q, const void* k_tensormap, const void* 
   const AttnPlan plan = attn_plan(rows, H, d, kv_len_max);
   const AttnWorkspace w = attn_workspace(workspace, H, d);
   const int G = plan.G;
-  const uint32_t* tab = w.table[plan.table_idx];
+  const bool e4m3 = k_exp != nullptr;
+  const uint32_t* tab = e4m3 ? nullptr : w.table[plan.table_idx];  // e4m3 launches have no calibrated split
   uint32_t* cta_ns = record_cta_ns ? w.cta_ns : nullptr;
   const float scale_log2 = scale * kLog2e;
   const __half* qh = (const __half*)q;
@@ -705,12 +807,18 @@ static int verify_attn_impl(const void* q, const void* k_tensormap, const void* 
   const uint8_t* pf_ptr = allow_pdl ? (const uint8_t*)next_weights : nullptr;
   const uint32_t pf_chunks = pf_ptr ? (uint32_t)(next_weight_bytes / kPfChunk) : 0u;
 
-  if (d == 128) {
-    if (rows <= 16) return launch_mma<128, 1, 3>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
-    return launch_mma<128, 2, 6>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
+#define TF_LAUNCH_MMA(KV_, D_, MT_, ST_)                                                                                            \
+  launch_mma<KV_, D_, MT_, ST_>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, \
+                                (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks, \
+                                k_exp, v_exp, cap)
+  // e4m3 tiles are half the bytes: twice the stages keep the same bytes in flight as the fp16 ring
+  if (e4m3) {
+    if (d == 128) return rows <= 16 ? TF_LAUNCH_MMA(__nv_fp8_e4m3, 128, 1, 6) : TF_LAUNCH_MMA(__nv_fp8_e4m3, 128, 2, 12);
+    return rows <= 16 ? TF_LAUNCH_MMA(__nv_fp8_e4m3, 64, 1, 8) : TF_LAUNCH_MMA(__nv_fp8_e4m3, 64, 2, 8);
   }
-  if (rows <= 16) return launch_mma<64, 1, 4>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
-  return launch_mma<64, 2, 4>(kmap, vmap, qh, layer, kv_len_host, kv_len_dev, R, H, grp, scale_log2, w.pm, w.pl, w.po, w.counters, (__half*)out, G, tree_mask, tree_cols, tab, cta_ns, clean_keys, allow_pdl, stream, pf_ptr, pf_chunks);
+  if (d == 128) return rows <= 16 ? TF_LAUNCH_MMA(__half, 128, 1, 3) : TF_LAUNCH_MMA(__half, 128, 2, 6);
+  return rows <= 16 ? TF_LAUNCH_MMA(__half, 64, 1, 4) : TF_LAUNCH_MMA(__half, 64, 2, 4);
+#undef TF_LAUNCH_MMA
 }
 
 // Measures the per-CTA streaming time of this very kernel on the caller's KV store and installs a split table
@@ -828,6 +936,21 @@ int tf_verify_attn_gqa(const void* q, const void* k_tensormap, const void* v_ten
   if (grp == 0) return TF_ERR_INVALID;
   return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hkv, grp, d, scale, out,
                           workspace, workspace_bytes, variant, nullptr, 0, false, clean_keys, stream);
+}
+
+int tf_verify_attn_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                        long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv,
+                        int d, float scale, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  const int grp = gqa_group(Hq, Hkv, "tf_verify_attn_e4m3");
+  if (grp == 0) return TF_ERR_INVALID;
+  TF_CHECK_ARG(k_exp && v_exp, "tf_verify_attn_e4m3: NULL exponent pointer");
+  TF_CHECK_ARG(cap > 0 && cap % TF_VERIFY_BOX_KEYS == 0, "tf_verify_attn_e4m3: cap (%lld) must be a positive multiple of %d", cap,
+               TF_VERIFY_BOX_KEYS);
+  TF_CHECK_ARG((((uintptr_t)k_exp | (uintptr_t)v_exp) & 15) == 0, "tf_verify_attn_e4m3: exponents must be 16-byte aligned");
+  TF_CHECK_ARG(kv_len_max <= cap && (kv_len_dev || kv_len_host <= cap), "tf_verify_attn_e4m3: kv_len (%d, max %d) exceeds cap %lld",
+               kv_len_host, kv_len_max, cap);
+  return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hkv, grp, d, scale, out,
+                          workspace, workspace_bytes, 0, nullptr, 0, false, 0, stream, nullptr, 0, k_exp, v_exp, cap);
 }
 
 int tf_verify_attn_prefetch(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,

@@ -22,7 +22,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._C import lib as _C_lib
-from .cache import FlashSimpleCache, RetrievalCache, StreamingLLMEvictionCache
+from .cache import FlashSimpleCache, RetrievalCache, StreamingLLMEvictionCache, kv_dtype_of, require_fp16_store
 from .config import LlamaShape
 from .rope import softmax_scale, tables_for
 
@@ -222,8 +222,8 @@ class LlamaModel:
         on an H100 the equal split is faster (full-KV verify at 124 944 keys: 0.684 ms equal vs 0.721-0.726 ms calibrated per
         layer) and, unlike a split measured at start-up, bit-reproducible across processes.  Short stores (< 16K keys) are left
         alone — there is nothing to balance."""
-        if os.environ.get("TRIFORCE_ATTN_CALIBRATE", "0") != "1" or self.is_draft or self.gqa:
-            return None
+        if os.environ.get("TRIFORCE_ATTN_CALIBRATE", "0") != "1" or self.is_draft or self.gqa or kv_dtype_of(kv_cache) != "fp16":
+            return None  # no calibrated split for GQA or E4M3 launches
         maps = kv_cache.tensor_maps
         cap = int(maps.shape[2])
         if cap < 16384:
@@ -310,27 +310,93 @@ class LlamaModel:
         h = self.embed_tokens[ids].contiguous()
         x = torch.empty_like(h)
         delta = None
+        for l in range(len(self.layers)):
+            delta = self._layer(l, h, delta, x, attn_fn)
+        return self._head(h, delta, x)
+
+    def _layer(self, l: int, h: torch.Tensor, delta, x: torch.Tensor, attn_fn):
+        """Decoder layer l on the n rows of the residual stream h (updated in place; x is scratch of h's shape): `delta` is the
+        previous layer's down_proj output (None before layer 0); returns this layer's."""
+        w = self.layers[l]
+        n = h.shape[0]
         stream = self.use_stream_linear and n <= ops.STREAM_MAX_ROWS  # per projection: a shard whose K is not a multiple of 64 keeps the fallback
-        for l, w in enumerate(self.layers):
-            self._add_norm(h, delta, w.ln1, x)
-            qkv = self._linear(x, w.wqkv, w.m_qkv if stream else None)
-            attn = attn_fn(l, qkv, n)
-            o = self._seam(attn.view(n, -1), w.wo, w.m_o if stream else None)
-            self._add_norm(h, o, w.ln2, x)
-            if stream and w.m_gu is not None:
-                if w.m_d is not None and w.m_d.K != self.local_inter:  # zero-padded down_proj (see _build_weight_maps)
-                    act = self._act_pad[:n]
-                    ops.stream_linear(x, w.m_gu, silu=True, out=act[:, :self.local_inter], workspace=self._linear_ws)
-                else:
-                    act = ops.stream_linear(x, w.m_gu, silu=True, workspace=self._linear_ws)
+        self._add_norm(h, delta, w.ln1, x)
+        qkv = self._linear(x, w.wqkv, w.m_qkv if stream else None)
+        attn = attn_fn(l, qkv, n)
+        o = self._seam(attn.view(n, -1), w.wo, w.m_o if stream else None)
+        self._add_norm(h, o, w.ln2, x)
+        if stream and w.m_gu is not None:
+            if w.m_d is not None and w.m_d.K != self.local_inter:  # zero-padded down_proj (see _build_weight_maps)
+                act = self._act_pad[:n]
+                ops.stream_linear(x, w.m_gu, silu=True, out=act[:, :self.local_inter], workspace=self._linear_ws)
             else:
-                gu = self._linear(x, w.wgu)
-                act = torch.empty((n, self.local_inter), dtype=torch.float16, device=self.device)
-                ops.silu_mul(gu, act)
-            m_d = w.m_d if (stream and w.m_d is not None and w.m_d.K == act.shape[1]) else None
-            delta = self._seam(act, w.wd, m_d)
+                act = ops.stream_linear(x, w.m_gu, silu=True, workspace=self._linear_ws)
+        else:
+            gu = self._linear(x, w.wgu)
+            act = torch.empty((n, self.local_inter), dtype=torch.float16, device=self.device)
+            ops.silu_mul(gu, act)
+        m_d = w.m_d if (stream and w.m_d is not None and w.m_d.K == act.shape[1]) else None
+        return self._seam(act, w.wd, m_d)
+
+    def _head(self, h: torch.Tensor, delta, x: torch.Tensor) -> torch.Tensor:
+        """Final norm + lm_head (fp32 logits) on the rows of h."""
+        stream = self.use_stream_linear and h.shape[0] <= ops.STREAM_MAX_ROWS
         self._add_norm(h, delta, self.norm, x)
         return self._linear(x, self.lm_head, self.m_lm_head if stream else None, out_fp32=True)
+
+    def _prefill_attention(self, q_out, maps, key_layer, value_layer, layer: int, kv_len: int, n: int, out, ws):
+        """Causal attention of n prompt rows over an fp16 store: verify kernel up to 32 rows, wgmma at d = 128, else library."""
+        if n <= ops.VERIFY_MAX_ROWS:
+            self._verify_attn(q_out, maps, layer, kv_len, n, out, ws)
+            return out
+        if self.head_dim == 128 and self.prefill_tc:
+            # prompt chunks on the wgmma kernel in causal mode (SURVEY §8 row f-2): no library call on the 7B / 13B path
+            self._tree_attn_tc(q_out, maps, layer, kv_len, n, None, 0, out, causal=True)
+            return out
+        return _prefill_attention_library(q_out, key_layer, value_layer, kv_len, self.scale)
+
+    def prefill_e4m3(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128) -> torch.Tensor:
+        """Prompt prefill into an E4M3 full-KV store, layer by layer, so that the prompt's causal attention never reads E4M3:
+        for each layer, every `chunk`-row piece runs through the layer with the ops and shapes of the chunk-major prefill
+        (`forward_target` on `chunk` ids at a time), appending its K/V to a one-layer fp16 scratch store with the fp16 RoPE
+        kernel and attending over it with the fp16 kernels; then the layer's rows are quantized into the E4M3 store.  The
+        residual stream of all prompt rows is kept between layers; logits are computed for the last piece only.  The logits
+        and the fp16 K/V rows are therefore bit-identical to the fp16 engine's chunk-major prefill with the same capacity."""
+        if kv_dtype_of(kv_cache) != "e4m3":
+            raise ValueError("prefill_e4m3 needs an E4M3 full-KV store")
+        if kv_cache.seq_len != 0:
+            raise NotImplementedError("the E4M3 prefill starts from an empty full-KV store (reset the cache first)")
+        ids = input_ids.reshape(-1)
+        N = ids.numel()
+        L, Hkv, cap, d = kv_cache.e4m3.shape
+        if N > cap:
+            raise ValueError(f"{N} prompt tokens exceed the {cap} slots of the full-KV store")
+        Hl = self.local_num_heads
+        h = self.embed_tokens[ids].contiguous()
+        delta = [None] * ((N + chunk - 1) // chunk)
+        x = torch.empty((min(chunk, N), h.shape[1]), dtype=torch.float16, device=self.device)
+        scratch_k = torch.zeros((1, Hkv, cap, d), dtype=torch.float16, device=self.device)
+        scratch_v = torch.zeros_like(scratch_k)
+        maps = ops.KVTensorMaps(scratch_k, scratch_v)
+        ws = self._workspace()
+        for l in range(L):
+            for i, c0 in enumerate(range(0, N, chunk)):
+                c1 = min(N, c0 + chunk)
+
+                def attn_fn(_l, qkv, n, c0=c0):
+                    q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
+                    out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
+                    self._rope_append(qkv, q_out, scratch_k[0], scratch_v[0], pos0=c0, slot0=c0)
+                    return self._prefill_attention(q_out, maps, scratch_k[0], scratch_v[0], 0, c0 + n, n, out, ws)
+
+                delta[i] = self._layer(l, h[c0:c1], delta[i], x[:c1 - c0], attn_fn)
+            ops.kv_quantize_e4m3(scratch_k[0], kv_cache.e4m3.k_codes[l], kv_cache.e4m3.k_exp[l], 0, N)
+            ops.kv_quantize_e4m3(scratch_v[0], kv_cache.e4m3.v_codes[l], kv_cache.e4m3.v_exp[l], 0, N)
+        del scratch_k, scratch_v, maps
+        c0 = (N - 1) // chunk * chunk
+        logits = self._head(h[c0:], delta[-1], x[:N - c0])
+        kv_cache.seq_len = N
+        return logits.unsqueeze(0)
 
     # --- target --------------------------------------------------------------------------------------------------------
     def forward_target(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, graph_cache: Optional[RetrievalCache] = None,
@@ -346,10 +412,29 @@ class LlamaModel:
             assert n == graph_cache.gamma + 1, "retrieval verify takes exactly gamma+1 rows (cache.py:186)"
             pos32 = position_ids.reshape(-1).to(torch.int32)
         old_len = kv_cache.seq_len
+        e4m3 = kv_dtype_of(kv_cache) == "e4m3"
+        if e4m3 and not spec and n > 2 * ops.VERIFY_MAX_ROWS:
+            raise ValueError(f"a {n}-row full-KV forward over an E4M3 store: prompts go through prefill_e4m3")
+        if e4m3:
+            ws = self._workspace()
 
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
+            if e4m3 and not spec:  # RoPE + quantized append, verify over the E4M3 store in bottom-right aligned row blocks
+                st, Hkv = kv_cache.e4m3, self.local_num_kv_heads
+                if use_device_len:
+                    kw = dict(pos0_dev=kv_cache.seq_len_dev, slot0_dev=kv_cache.seq_len_dev)
+                elif position_ids is not None:
+                    kw = dict(pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=old_len)
+                else:
+                    kw = dict(pos0=old_len, slot0=old_len)
+                ops.rope_append_e4m3(qkv, Hl, Hkv, d, self.cos, self.sin, q_out, st, l, **kw)
+                if build:
+                    qs[l] = q_out[0]
+                ops.verify_attn_e4m3(q_out, st, l, n if use_device_len else old_len + n, n, Hl, Hkv, d, self.scale, out, ws,
+                                     kv_len_dev=kv_cache.seq_len_dev if use_device_len else None)
+                return out
             if spec:
                 self._rope_append(qkv, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
                                   slot0=graph_cache.max_budget)
@@ -369,14 +454,8 @@ class LlamaModel:
                 self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos0=old_len, slot0=old_len)
             if build:
                 qs[l] = q_out[0]
-            if n <= ops.VERIFY_MAX_ROWS:
-                self._verify_attn(q_out, kv_cache.tensor_maps, l, old_len + n, n, out, ws)
-                return out
-            if d == 128 and self.prefill_tc:
-                # prompt chunks on the wgmma kernel in causal mode (SURVEY §8 row f-2): no library call on the 7B / 13B path
-                self._tree_attn_tc(q_out, kv_cache.tensor_maps, l, old_len + n, n, None, 0, out, causal=True)
-                return out
-            return _prefill_attention_library(q_out, kv_cache.key_store[l], kv_cache.value_store[l], old_len + n, self.scale)
+            return self._prefill_attention(q_out, kv_cache.tensor_maps, kv_cache.key_store[l], kv_cache.value_store[l], l,
+                                           old_len + n, n, out, ws)
 
         logits = self._stack(input_ids, attn_fn)
         if not spec and not use_device_len:
@@ -389,7 +468,10 @@ class LlamaModel:
                 for l in range(L):
                     seq = old_len + (1 if l == L - 1 else 0)
                     m = seq - graph_cache.prefill
-                    if m > 0:
+                    if m > 0 and e4m3:
+                        ops.tail_update_e4m3(kv_cache.e4m3, graph_cache.key_store, graph_cache.value_store, graph_cache.prefill,
+                                             graph_cache.max_budget, seq, layer0=l, n_layers=1)
+                    elif m > 0:
                         B, P = graph_cache.max_budget, graph_cache.prefill
                         graph_cache.key_store[l, :, B - m:B] = kv_cache.key_store[l, :, P:seq]
                         graph_cache.value_store[l, :, B - m:B] = kv_cache.value_store[l, :, P:seq]
@@ -437,6 +519,7 @@ class LlamaModel:
     def forward_tree_verify(self, input_ids: torch.Tensor, kv_cache, position_ids: torch.Tensor, mask_bits: torch.Tensor) -> torch.Tensor:
         """The masked verify of all T tree nodes over the FULL KV (SpecTree_TP.py:168-175 → TP_llama_tree `inference` with an
         attention mask): nodes are appended at slots [seq_len, seq_len + T) and see the whole prefix plus their ancestors."""
+        require_fp16_store(kv_cache, "forward_tree_verify")
         Hl, d = self.local_num_heads, self.head_dim
         pos32 = position_ids.reshape(-1).to(torch.int32)
         T = input_ids.numel()

@@ -48,6 +48,133 @@ class KVTensorMaps:
         self.shape = (L, H, cap, d)
 
 
+class E4m3Store:
+    """One E4M3 full-KV store (the format of include/triforce_b200.h): codes uint8 [L,Hkv,cap,d] and exponents int8 [L,Hkv,cap],
+    for K and for V, plus the TMA descriptors of the codes.  cap must be a multiple of VERIFY_BOX_KEYS."""
+
+    def __init__(self, k_codes: torch.Tensor, v_codes: torch.Tensor, k_exp: torch.Tensor, v_exp: torch.Tensor):
+        require_cuda(k_codes, v_codes, k_exp, v_exp)
+        L, H, cap, d = k_codes.shape
+        for t in (k_codes, v_codes):
+            assert t.dtype == torch.uint8 and t.is_contiguous() and t.shape == (L, H, cap, d)
+        for t in (k_exp, v_exp):
+            assert t.dtype == torch.int8 and t.is_contiguous() and t.shape == (L, H, cap)
+        if cap % VERIFY_BOX_KEYS:
+            raise ValueError(f"an e4m3 store needs a capacity that is a multiple of {VERIFY_BOX_KEYS}, got {cap}")
+        self.k_codes, self.v_codes, self.k_exp, self.v_exp = k_codes, v_codes, k_exp, v_exp
+        self.k = (ctypes.c_uint8 * 128)()
+        self.v = (ctypes.c_uint8 * 128)()
+        for buf, t in ((self.k, k_codes), (self.v, v_codes)):
+            check(lib().tf_kv_tensormap_encode_e4m3(ctypes.addressof(buf), t.data_ptr(), d, cap, H, L, t.stride(1), t.stride(0),
+                                                    VERIFY_BOX_KEYS), "tf_kv_tensormap_encode_e4m3")
+        self.k_ptr = ctypes.addressof(self.k)
+        self.v_ptr = ctypes.addressof(self.v)
+        self.shape = (L, H, cap, d)
+
+    @staticmethod
+    def empty(L: int, H: int, cap: int, d: int, device) -> "E4m3Store":
+        return E4m3Store(torch.zeros((L, H, cap, d), dtype=torch.uint8, device=device),
+                         torch.zeros((L, H, cap, d), dtype=torch.uint8, device=device),
+                         torch.zeros((L, H, cap), dtype=torch.int8, device=device),
+                         torch.zeros((L, H, cap), dtype=torch.int8, device=device))
+
+
+def kv_quantize_e4m3(src_layer: torch.Tensor, codes_layer: torch.Tensor, exp_layer: torch.Tensor, slot0: int, n: int):
+    """fp16 rows [slot0, slot0+n) of src_layer [Hkv, >=cap, d] -> the same slots of one layer of K or V codes [Hkv, cap, d]
+    and exponents [Hkv, cap] (tf_kv_quantize_e4m3)."""
+    require_cuda(src_layer, codes_layer, exp_layer)
+    _f16c(src_layer, "src_layer")
+    H, cap, d = codes_layer.shape
+    assert codes_layer.dtype == torch.uint8 and codes_layer.is_contiguous()
+    assert exp_layer.dtype == torch.int8 and exp_layer.is_contiguous() and exp_layer.shape == (H, cap)
+    assert src_layer.shape[0] == H and src_layer.shape[2] == d and src_layer.stride(2) == 1 and src_layer.stride(1) == d
+    check(lib().tf_kv_quantize_e4m3(src_layer.data_ptr(), src_layer.stride(0), slot0, n, H, d, codes_layer.data_ptr(),
+                                    exp_layer.data_ptr(), cap, stream_ptr()), "tf_kv_quantize_e4m3")
+    COUNTER.n += 1
+
+
+def rope_append_e4m3(qkv: torch.Tensor, Hq: int, Hkv: int, d: int, cos, sin, q_out, store: E4m3Store, layer: int, *,
+                     pos_ids=None, pos0: int = 0, pos0_dev=None, slot0: int = 0, slot0_dev=None):
+    """rope_append_gqa with the appended K/V rows quantized into `layer` of the e4m3 store (tf_rope_append_e4m3)."""
+    require_cuda(qkv, cos, sin, q_out)
+    _f16c(qkv, "qkv")
+    R = qkv.shape[0]
+    L, H, cap, _ = store.shape
+    assert H == Hkv and qkv.stride(1) == 1 and qkv.shape[1] == (Hq + 2 * Hkv) * d
+    assert q_out.is_contiguous() and q_out.shape == (R, Hq, d)
+    base = qkv.data_ptr()
+    es = qkv.element_size()
+    if pos_ids is not None:
+        assert pos_ids.dtype == torch.int32 and pos_ids.numel() >= R
+    check(lib().tf_rope_append_e4m3(base, base + Hq * d * es, base + (Hq + Hkv) * d * es, qkv.stride(0), cos.data_ptr(),
+                                    sin.data_ptr(), cos.shape[0], ptr(pos_ids), pos0, ptr(pos0_dev), slot0, ptr(slot0_dev), R, Hq,
+                                    Hkv, d, q_out.data_ptr(), store.k_codes[layer].data_ptr(), store.v_codes[layer].data_ptr(),
+                                    store.k_exp[layer].data_ptr(), store.v_exp[layer].data_ptr(), cap, stream_ptr()),
+          "tf_rope_append_e4m3")
+    COUNTER.n += 1
+
+
+def verify_attn_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float, out,
+                     workspace, kv_len_dev=None, kv_len_max: Optional[int] = None):
+    """verify_attn_gqa (causal, Hq == Hkv is MHA) over the e4m3 store (tf_verify_attn_e4m3); workspace from
+    verify_attn_gqa_workspace.  Rows are cut into bottom-right aligned blocks of gqa_row_block(Hq, Hkv) token rows."""
+    require_cuda(q, out, workspace)
+    _f16c(q, "q")
+    assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and out.shape == q.shape
+    L, H, cap, _ = store.shape
+    assert H == Hkv, (store.shape, Hkv)
+    if kv_len_max is None:
+        kv_len_max = cap if kv_len_dev is not None else kv_len
+    step = gqa_row_block(Hq, Hkv)
+    if step < 1:
+        raise ValueError(f"{Hq // Hkv} query heads per KV head exceed the {VERIFY_MAX_ROWS} rows of a verify-attention CTA")
+    for r0 in range(0, R, step):
+        r1 = min(R, r0 + step)
+        check(lib().tf_verify_attn_e4m3(q[r0:r1].data_ptr(), store.k_ptr, store.v_ptr, store.k_exp.data_ptr(), store.v_exp.data_ptr(),
+                                        cap, layer, kv_len - (R - r1), ptr(kv_len_dev), min(kv_len_max, cap), r1 - r0, Hq, Hkv, d,
+                                        scale, out[r0:r1].data_ptr(), workspace.data_ptr(), workspace.numel(), stream_ptr()),
+              "tf_verify_attn_e4m3")
+        COUNTER.n += 1
+
+
+def retrieval_build_e4m3(store: E4m3Store, q, retr_key_store, retr_value_store, prefill: int, chunk: int, budget: int,
+                         layer0: int = 0, n_layers: Optional[int] = None, out_idx=None, out_scores=None):
+    """retrieval_build / retrieval_build_gqa ("group_sum" when Hq > Hkv) over the e4m3 store (tf_retrieval_build_e4m3):
+    q [n_layers,Hq,d]; the gather writes D into the fp16 retrieval store."""
+    require_cuda(q, retr_key_store, retr_value_store)
+    L, Hkv, cap, d = store.shape
+    n = q.shape[0] if n_layers is None else n_layers
+    Hq = q.shape[1]
+    _f16c(q, "q")
+    assert q.is_contiguous() and q.shape == (n, Hq, d), (q.shape, (n, Hq, d))
+    ws_bytes = lib().tf_retrieval_build_workspace_bytes(n, Hkv, d, prefill, chunk, budget)
+    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=q.device)
+    if out_idx is not None:
+        assert out_idx.dtype == torch.int32 and out_idx.is_contiguous() and out_idx.shape == (n, Hkv, budget // chunk)
+    if out_scores is not None:
+        assert out_scores.dtype == torch.float16 and out_scores.is_contiguous() and out_scores.shape == (n, Hkv, prefill // chunk)
+    kc = store.k_codes
+    check(lib().tf_retrieval_build_e4m3(kc[layer0].data_ptr(), store.v_codes[layer0].data_ptr(), store.k_exp[layer0].data_ptr(),
+                                        store.v_exp[layer0].data_ptr(), kc.stride(0), kc.stride(1), q.data_ptr(), n, Hq, Hkv, d,
+                                        prefill, chunk, budget, retr_key_store[layer0].data_ptr(), retr_value_store[layer0].data_ptr(),
+                                        retr_key_store.stride(0), retr_key_store.stride(1), ptr(out_idx), ptr(out_scores),
+                                        ws.data_ptr(), ws.numel(), stream_ptr()), "tf_retrieval_build_e4m3")
+    COUNTER.n += 3
+
+
+def tail_update_e4m3(store: E4m3Store, retr_key_store, retr_value_store, prefill: int, budget: int, seq_len: int,
+                     seq_len_dev=None, max_new: int = 0, layer0: int = 0, n_layers: Optional[int] = None):
+    """tail_update from the e4m3 store into the fp16 retrieval store (tf_tail_update_e4m3), layers [layer0, layer0+n): writes D."""
+    L, H, cap, d = store.shape
+    n = L - layer0 if n_layers is None else n_layers
+    kc = store.k_codes
+    check(lib().tf_tail_update_e4m3(kc[layer0].data_ptr(), store.v_codes[layer0].data_ptr(), store.k_exp[layer0].data_ptr(),
+                                    store.v_exp[layer0].data_ptr(), kc.stride(0), kc.stride(1), retr_key_store[layer0].data_ptr(),
+                                    retr_value_store[layer0].data_ptr(), retr_key_store.stride(0), retr_key_store.stride(1), n, H, d,
+                                    prefill, budget, seq_len, ptr(seq_len_dev), max_new, stream_ptr()), "tf_tail_update_e4m3")
+    COUNTER.n += 1
+
+
 def retrieval_build(key_store, value_store, q, retr_key_store, retr_value_store, prefill: int, chunk: int, budget: int,
                     layer0: int = 0, n_layers: Optional[int] = None, out_idx=None, out_scores=None):
     """key_store/value_store [L,H,cap,d]; q [n_layers,H,d]; retr_* [L,H,rcap,d].  Builds layers [layer0, layer0+n)."""

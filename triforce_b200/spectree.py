@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .cache import require_fp16_store
 from .rng import TorchNoise
 from .sampling import norm_logits
 
@@ -98,6 +99,7 @@ def build_sampling(grow_map: Dict, temperature: float, device):
 class SpecTree:
     def __init__(self, engine, temperature: float = 0.6, top_p: float = 0.9, max_length=256, vocab_size=32000, grow_map=None,
                  residual_graph=None, sampling_callables=None, sample_gather_indices=None, tokenizer=None, noise=None) -> None:
+        require_fp16_store(getattr(engine, "kv_cache", None), "SpecTree (the Sequoia tree path)")
         self.graph_engine = engine
         self.temperature, self.top_p = temperature, top_p
         self.residual_graph = residual_graph or get_residual
