@@ -368,9 +368,10 @@ int tf_skinny_gemm_allreduce(const void* x, long long x_row_stride, const void* 
  * tf_loop_graph_build makes  pre -> WHILE(n < gamma){ body; cudaGraphSetConditional } -> post  out of them.
  * state int32[8]: [0] n, [1] k = ids emitted, [2] last accept, [3] accepted draft tokens, [4] inner iterations.
  * rng: device struct {uint64 seed, uint64 next_draw} — counter-based Philox4x32-10; draw c, element i -> lane i%4 of
- *   Philox(counter = (i/4, c_lo, c_hi, 0), key = seed); uniform in (0,1), exponential = -log(uniform).  Order of draws = the
- *   reference's: per inner iteration exponential / uniform / exponential, per outer iteration a uniform block then (when a token is
- *   drawn) one exponential.  tf_philox_fill(state, kind 0 uniform | 1 exponential) replays one draw into a buffer and advances the
+ *   Philox(counter = (i/4, c_lo, c_hi, 0), key = seed); uniform = ((x >> 8) + 1/2) * 2^-24 in float32, strictly inside (0,1)
+ *   (the one word that rounds to 1.0 gives 1 - 2^-24), exponential = -log(uniform).  Order of draws = the reference's: per inner
+ *   iteration exponential / uniform / exponential, per outer iteration a uniform block then (when a token is drawn) one
+ *   exponential.  tf_philox_fill(state, kind 0 uniform | 1 exponential) replays one draw into a buffer and advances the
  *   counter — the step-wise loop uses it, which is how both loops are compared event for event.
  * tf_loop_verify: res int32[16]: [0] tokens produced, [1] accepted ids, [2] rejected, [3] gamma2, [4] examined, [5] hit eos,
  *   [6] inner iterations, [7] inner accepts, [8] draft-window shift, [9] new seq_len; it also advances *seq_len_dev by count + 1 and

@@ -14,9 +14,9 @@
 // graph and reads ONE small result record.
 //
 // Random numbers: draw `c` of stream (seed) = Philox4x32-10(counter = (element / 4, c_lo, c_hi, 0), key = seed); element i takes
-// lane i % 4.  Uniforms u in (0, 1); exponentials -log(u).  The consumption order is the reference's (decoding.py:185,192,201/212,
-// 98,114/130): per inner iteration exponential (draft sample), uniform, exponential (accept / resample); per outer iteration one
-// block of uniforms, then one exponential when a token is drawn.  `tf_philox_fill` replays the same draws for the step-wise
+// lane i % 4.  Uniforms u strictly inside (0, 1) (philox_to_uniform); exponentials -log(u) > 0.  The consumption order is the
+// reference's (decoding.py:185,192,201/212,98,114/130): per inner iteration exponential (draft sample), uniform, exponential
+// (accept / resample); per outer iteration one block of uniforms, then one exponential when a token is drawn.  `tf_philox_fill` replays the same draws for the step-wise
 // (host-driven) loop, which is how the two loops are checked against each other event for event.
 #include <float.h>
 #include <string.h>
@@ -44,10 +44,16 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   }
   return c;
 }
+// Philox word -> uniform in (0, 1): (top 24 bits + 1/2) * 2^-24.  Above 2^23 the float sum is a tie that rounds to even, so the
+// word 0xFFFFFF.. would give exactly 1.0, whose -log is -0.0 (p / -0 is NaN for p = 0, and NaN wins the sampling argmax).  That
+// one value becomes 1 - 2^-24, which the rounded sum never produces: every other word keeps its bits.
+__device__ __forceinline__ float philox_to_uniform(uint32_t x) {
+  const float u = ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f);
+  return u < 1.0f ? u : __uint_as_float(0x3f7fffffu);
+}
 __device__ __forceinline__ float philox_uniform(unsigned long long seed, unsigned long long draw, uint32_t elem) {
   const uint4 r = philox4x32_10(make_uint4(elem >> 2, (uint32_t)draw, (uint32_t)(draw >> 32), 0u), make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-  const uint32_t x = (elem & 3u) == 0 ? r.x : ((elem & 3u) == 1 ? r.y : ((elem & 3u) == 2 ? r.z : r.w));
-  return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0, 1); same formula as philox_to_uniform
+  return philox_to_uniform((elem & 3u) == 0 ? r.x : ((elem & 3u) == 1 ? r.y : ((elem & 3u) == 2 ? r.z : r.w)));
 }
 __device__ __forceinline__ float philox_exponential(unsigned long long seed, unsigned long long draw, uint32_t elem) {
   return -logf(philox_uniform(seed, draw, elem));
@@ -63,7 +69,6 @@ __device__ __forceinline__ bool loop_better(float v, int i, float bv, int bi) { 
   if (vn && bn) return i < bi;
   return v > bv || (v == bv && i < bi);
 }
-__device__ __forceinline__ float philox_to_uniform(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
 // argmax_i num(i) / Exp_i over [0, V) with Exp_i = exponential `draw` of the stream; every thread returns the winner.
 // One Philox call serves the four elements 4g .. 4g+3 (the same element -> lane mapping as philox_uniform).
 template <typename F>
