@@ -312,6 +312,34 @@ size_t tf_stream_linear_workspace_bytes(void);
 int tf_stream_linear(const void* x, long long x_row_stride, const void* w_tensormap, int M, int N, int K, int epilogue, void* y,
                      long long y_row_stride, void* workspace, size_t workspace_bytes, tf_stream_t stream);
 
+/* ---- E4M3 projection weights (opt-in; fp16 stays the default) ------------------------------------------------------
+ * A projection matrix W [N][K] (one row per output feature) is stored as
+ *   codes     uint8 [N][K] (torch.float8_e4m3fn bits), row-major like the fp16 matrix, row stride in bytes (% 16 == 0);
+ *   exponents int8  [N], one per row.
+ * Row w: e = max(-15, the smallest integer with max|w| <= 448 * 2^e) (0 for an all-zero row); code = e4m3_rn(w / 2^e), round to
+ * nearest even.  The row stands for D = code * 2^e, which is an exact fp16 value (codes are multiples of 2^-9 with at most 4
+ * significant bits, and e >= -15): nothing rounds in D.  Rows that are not finite or have max|w| > 61440 = 240 * 2^8 (above
+ * which D can round past the fp16 maximum) are refused.
+ * tf_weight_quantize_e4m3: W fp16 [N][row_stride elements] -> codes and exponents.  A refused row is left unwritten and counted
+ *   into *refused_rows (device int32, may be NULL); the caller reads the count after the stream is synchronised.
+ * tf_weight_dequantize_e4m3: codes and exponents -> D fp16 [N][d_row_stride elements] (the GEMM path of > 24-row forwards).
+ * tf_weight_tensormap_encode_e4m3: the descriptor of a code matrix for tf_stream_linear_e4m3 (one view for every epilogue).
+ * tf_stream_linear_e4m3: tf_stream_linear over E4M3 weights, epilogues 0, 1 and 2 (no TP seams), same M / K / alignment checks,
+ *   workspace and PDL bit.  The same kernel with 8 KB code stages: a lane converts the codes of its k slots with
+ *   cvt.rn.f16x2.e4m3x2 once for all token blocks, and the epilogue multiplies each row's fp32 sum by its 2^e (the gate and the
+ *   up row each by their own) before the fp16 rounding.  As D is exact and power-of-two scaling commutes with the fp32 products
+ *   and sums, y is BIT-IDENTICAL to tf_stream_linear on D for every M <= 24 and epilogue.  Exception measured on H100: rows
+ *   whose D is almost entirely fp16 subnormals (max|w| around 2^-10 and below) can differ in the last bit of a few small
+ *   outputs, because the fp16 kernel's tensor-core sums over subnormal operands are not exactly 2^e times the e4m3 kernel's.
+ */
+int tf_weight_quantize_e4m3(const void* W, long long row_stride, int N, int K, void* codes, long long codes_row_stride, int8_t* exps,
+                            int32_t* refused_rows, tf_stream_t stream);
+int tf_weight_dequantize_e4m3(const void* codes, long long codes_row_stride, const int8_t* exps, int N, int K, void* D, long long d_row_stride,
+                              tf_stream_t stream);
+int tf_weight_tensormap_encode_e4m3(void* out_128B, const void* codes, int N, int K, long long row_stride);
+int tf_stream_linear_e4m3(const void* x, long long x_row_stride, const void* w_tensormap, const int8_t* w_exp, int M, int N, int K,
+                          int epilogue, void* y, long long y_row_stride, void* workspace, size_t workspace_bytes, tf_stream_t stream);
+
 /* tf_stream_linear_allreduce: the TP seams as ONE kernel — the row-parallel o_proj / down_proj of tf_stream_linear AND the
  *   all-reduce(SUM) that follows it in the reference (models/tensor_op.py:176-179, 357-359): y = sum_r x_r · W_r^T, fp16, identical
  *   bits on every rank.  The reducer warp of each finished [16 features x M tokens] tile stores its fp16 partial into slot `rank`

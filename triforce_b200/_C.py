@@ -84,6 +84,11 @@ _SIGNATURES = {
     "tf_stream_linear_workspace_bytes": (c_size_t, []),
     "tf_stream_linear": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p, c_size_t,
                                  c_void_p]),
+    "tf_weight_quantize_e4m3": (c_int, [c_void_p, c_longlong, c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p]),
+    "tf_weight_dequantize_e4m3": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p, c_longlong, c_void_p]),
+    "tf_weight_tensormap_encode_e4m3": (c_int, [c_void_p, c_void_p, c_int, c_int, c_longlong]),
+    "tf_stream_linear_e4m3": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p,
+                                      c_size_t, c_void_p]),
     "tf_stream_linear_allreduce_buffer_bytes": (c_size_t, []),
     "tf_stream_linear_allreduce": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p, c_size_t,
                                            c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

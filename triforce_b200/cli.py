@@ -53,6 +53,9 @@ FLAGS = {
         ("--seed", dict(type=int, default=0)),
         ("--kv_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
                             help="full-KV store: fp16, or FP8 E4M3 with a per-row power-of-two scale (changes the target's numerics)")),
+        ("--weight_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
+                                help="target projection weights: fp16, or FP8 E4M3 with a per-row power-of-two scale "
+                                     "(changes the target's numerics)")),
     ],
     "offloading_TP": _COMMON_TP_FLAGS + [("--gamma", dict(type=str, default=6))],
     "offloading_seqouia": _COMMON_TP_FLAGS + [("--tree_size", dict(type=str, default="512"))],
@@ -119,7 +122,7 @@ def run_on_chip(argv: Optional[List[str]] = None) -> None:
     # no checkpoints offline: a hub id means seeded random-init weights of that architecture, stated explicitly (and printed)
     tpath, dpath = args.target_path or HUB_NAMES[args.target], args.draft_path or "JackFram/llama-68m"
     target = TargetLlamaForCausalLM.from_pretrained(tpath, torch_dtype=torch.float16, device_map="cuda:0", seed=1,
-                                                    synthetic=not os.path.isdir(tpath)).eval()
+                                                    synthetic=not os.path.isdir(tpath), weight_dtype=args.weight_dtype).eval()
     draft = DraftLlamaForCausalLM.from_pretrained(dpath, torch_dtype=torch.float16, device_map="cuda:0", seed=2,
                                                   synthetic=not os.path.isdir(dpath)).eval()
     tokenizer = SyntheticTokenizer()

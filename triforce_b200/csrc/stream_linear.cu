@@ -51,6 +51,10 @@
 // (bit-identical to all-reduce-then-add) and goes on with the residual add and the RMSNorm; it also advances the epoch.
 #include <string.h>
 
+#include <type_traits>
+
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 
 namespace tf {
@@ -78,6 +82,15 @@ constexpr int kSlKC = 512;                                // k elements per stag
 constexpr uint32_t kSlWBytes = kSlRows * kSlKC * 2;       // 16 KB of weights per stage
 constexpr uint32_t kSlXBytes = 8 * kSlKC * 2;             // 8 KB of x per token block per stage
 constexpr int kSlMaxStages = 8;
+// E4M3 weights (stream_linear_kernel<MT, __nv_fp8_e4m3>): a stage carries the codes of the same 16 rows x 512 k, 8 KB, and the
+// ring may hold more stages in the same shared memory
+constexpr uint32_t kSlWBytesE4 = kSlRows * kSlKC;
+constexpr int kSlMaxStagesE4 = 12;
+template <typename WT> struct SlW {
+  static constexpr bool kE4 = std::is_same<WT, __nv_fp8_e4m3>::value;
+  static constexpr uint32_t kBytes = kE4 ? kSlWBytesE4 : kSlWBytes;
+  static constexpr int kMaxStages = kE4 ? kSlMaxStagesE4 : kSlMaxStages;
+};
 constexpr size_t kSlSmemTwoPerSM = 233472 / 2 - 1024;     // dynamic shared memory that still lets two CTAs share an SM
 constexpr size_t kSlSmemOnePerSM = 232448;                // 227 KB opt-in maximum
 
@@ -108,6 +121,7 @@ struct StreamArgs {
   float4* part;             // [grid][MT][32 lanes]: the k-steps of a cut tile computed by the right-hand neighbour
   int* flags;               // [grid]: part[b] published (zero between launches)
   StreamPeers peers;        // epilogue 3 only
+  const int8_t* wexp;       // E4M3 weights: one exponent per weight row (stream_linear_kernel<MT, __nv_fp8_e4m3> only)
 };
 
 __device__ __forceinline__ void sl_st_release_sys(int* p, int v) { asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
@@ -128,18 +142,21 @@ __device__ __forceinline__ void sl_multimem_st_v4(void* mc, uint4 v) {  // one s
   asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(mc), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
-// MT = token blocks of 8 rows (1: M <= 8, 2: M <= 16, 3: M <= 24).
-template <int MT>
+// MT = token blocks of 8 rows (1: M <= 8, 2: M <= 16, 3: M <= 24).  WT = the weight element: __half, or __nv_fp8_e4m3 for
+// E4M3 weights (codes through wmap, exponents a.wexp; see "E4M3 weights" at tf_stream_linear_e4m3).
+template <int MT, typename WT = __half>
 __global__ void __launch_bounds__(kSlThreads, MT == 1 ? 2 : 1)
     stream_linear_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap xmap, const StreamArgs a) {
   extern __shared__ uint8_t sl_smem_raw[];
-  constexpr uint32_t kStage = kSlWBytes + MT * kSlXBytes;
+  constexpr bool kE4 = SlW<WT>::kE4;
+  constexpr uint32_t kWBytes = SlW<WT>::kBytes;
+  constexpr uint32_t kStage = kWBytes + MT * kSlXBytes;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sl_smem_raw) + 1023) & ~(uintptr_t)1023);
   const int stages = a.stages;
   uint8_t* ring = smem;                                                              // [stages][W 16 KB | x MT * 8 KB]
   float4* red = reinterpret_cast<float4*>(ring + (size_t)stages * kStage);           // [2][MT][8 warps][32 lanes]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(red + 2 * MT * kSlWarps * 32);
-  uint64_t* empty_bar = full_bar + kSlMaxStages;
+  uint64_t* empty_bar = full_bar + SlW<WT>::kMaxStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = a.epilogue == 1 ? (a.N / 2 + 7) / 8 : (a.N + kSlRows - 1) / kSlRows;
@@ -166,6 +183,18 @@ __global__ void __launch_bounds__(kSlThreads, MT == 1 ? 2 : 1)
       auto load_w = [&](int u, uint32_t s) {
         const int tile = u / ksteps, ks = u - tile * ksteps;
         const uint32_t dst = ring_u + s * kStage;
+        if constexpr (kE4) {
+          // codes seen as (32 bytes, rows, K/32): a box [32, 8, 8] is 8 rows x 256 k, laid out [k-block of 32][row][32 bytes]
+          const int kq0 = ks * (kSlKC / 32);
+#pragma unroll
+          for (int half = 0; half < 2; ++half)
+#pragma unroll
+            for (int rg = 0; rg < 2; ++rg) {
+              const int row0 = a.epilogue == 1 ? (rg == 0 ? tile * 8 : inter + tile * 8) : tile * kSlRows + rg * 8;
+              sl_tma_3d(dst + half * (kWBytes / 2) + rg * (kWBytes / 4), &wmap, &full_bar[s], 0, row0, kq0 + half * 8);
+            }
+          return;
+        }
         const int kb0 = ks * (kSlKC / 64);
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -180,7 +209,7 @@ __global__ void __launch_bounds__(kSlThreads, MT == 1 ? 2 : 1)
       };
       auto load_x = [&](int u, uint32_t s) {
         const int tile = u / ksteps, ks = u - tile * ksteps;
-        const uint32_t dst = ring_u + s * kStage + kSlWBytes;
+        const uint32_t dst = ring_u + s * kStage + kWBytes;
         const int kb0 = ks * (kSlKC / 64);
 #pragma unroll
         for (int b = 0; b < MT; ++b)
@@ -230,9 +259,42 @@ __global__ void __launch_bounds__(kSlThreads, MT == 1 ? 2 : 1)
       const uint32_t s = it % (uint32_t)stages, ph = (it / (uint32_t)stages) & 1u;
       mbar_wait(&full_bar[s], ph);
       const uint32_t wst = ring_u + s * kStage;
-      const uint32_t xst = wst + kSlWBytes;
+      const uint32_t xst = wst + kWBytes;
 #pragma unroll
       for (int cc = 0; cc < 2; ++cc) {
+        if constexpr (kE4) {
+          // the same chunk and k slots as below; lane (g, t) takes the 8 code bytes k = 32c + 8t .. +7 of rows g and g+8
+          // from [half 4 KB][row group 2 KB][k-block c & 7][row & 7][32 bytes]: the 16 lanes of a half warp read 128
+          // consecutive bytes (conflict-free LDS.64), and each code is converted once for all MT token blocks
+          const int c = warp + cc * kSlWarps;
+          const uint32_t half = (uint32_t)c >> 3, kq = (uint32_t)c & 7u;
+          const uint32_t wa_addr = wst + half * (kWBytes / 2) + (kq * 8u + (uint32_t)g) * 32u + (uint32_t)t * 8u;
+          uint2 ca, cb;
+          asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(ca.x), "=r"(ca.y) : "r"(wa_addr));
+          asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(cb.x), "=r"(cb.y) : "r"(wa_addr + kWBytes / 4));
+          uint4 wa, wb;
+          {
+            __half2 h;
+            h = kv_e4m3_codes2((uint16_t)(ca.x & 0xffffu)); wa.x = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(ca.x >> 16));     wa.y = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(ca.y & 0xffffu)); wa.z = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(ca.y >> 16));     wa.w = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(cb.x & 0xffffu)); wb.x = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(cb.x >> 16));     wb.y = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(cb.y & 0xffffu)); wb.z = *reinterpret_cast<uint32_t*>(&h);
+            h = kv_e4m3_codes2((uint16_t)(cb.y >> 16));     wb.w = *reinterpret_cast<uint32_t*>(&h);
+          }
+          // x keeps the fp16 layout of the fp16 kernel (the same line / swizzle arithmetic)
+          const uint32_t kb = ((uint32_t)c & 7u) >> 1, j = (((uint32_t)c & 1u) << 2) + (uint32_t)t;
+          const uint32_t la = 4u * (uint32_t)g + kb;
+#pragma unroll
+          for (int b = 0; b < MT; ++b) {
+            const uint4 xa = sl_lds128(xst + (uint32_t)(b * 2 + (int)half) * (kSlXBytes / 2) + la * 128u + ((j ^ (la & 7u)) << 4));
+            sl_mma(acc[b], wa.x, wb.x, wa.y, wb.y, xa.x, xa.y);
+            sl_mma(acc[b], wa.z, wb.z, wa.w, wb.w, xa.z, xa.w);
+          }
+          continue;
+        }
         // chunk c of the stage = 32 k; lane (g, t) takes the 16 bytes k = 32c + 8t .. +7 of weight rows g and g+8 and of token
         // row g.  Inside a box the 128-byte line of (row r, k-block kb) is line L = 4r + kb, its 16-byte piece j at j ^ (L & 7).
         const int c = warp + cc * kSlWarps;
@@ -388,7 +450,17 @@ __global__ void __launch_bounds__(kSlThreads, MT == 1 ? 2 : 1)
 #pragma unroll
       for (int b = 0; b < MT; ++b) {
         if (second_half || a.epilogue >= 3) continue;
-        const float4 sum = sums[b];
+        float4 sum = sums[b];
+        if constexpr (kE4) {
+          // the row's 2^e on the whole sum (the neighbour's partial included), before the fp16 rounding of the fp16 kernel:
+          // code * 2^e is D exactly and power-of-two scaling commutes with the fp32 products and sums, so y is the fp16
+          // kernel's y on D bit for bit (except rows whose D is almost all fp16 subnormals, see tf_stream_linear_e4m3)
+          const int r_lo = a.epilogue == 1 ? tile * 8 + g : tile * kSlRows + g;
+          const int r_hi = a.epilogue == 1 ? inter + tile * 8 + g : r_lo + 8;
+          const float s_lo = kv_e4m3_pow2(r_lo < (a.epilogue == 1 ? inter : a.N) ? (int)a.wexp[r_lo] : 0);
+          const float s_hi = kv_e4m3_pow2(r_hi < a.N && (a.epilogue != 1 || tile * 8 + g < inter) ? (int)a.wexp[r_hi] : 0);
+          sum.x *= s_lo; sum.y *= s_lo; sum.z *= s_hi; sum.w *= s_hi;
+        }
         // accumulator layout: (x, y) = weight row g, tokens 2t, 2t+1; (z, w) = weight row g+8, same tokens
         const int tok0 = b * 8 + 2 * t, tok1 = tok0 + 1;
         if (a.epilogue == 1) {
@@ -454,9 +526,10 @@ struct StreamPlan {
   int stages, ctas_per_sm;
   size_t smem;
 };
+template <typename WT = __half>
 static StreamPlan stream_plan(int MT) {
-  const size_t stage = kSlWBytes + (size_t)MT * kSlXBytes;
-  const size_t fixed = 1024 + (size_t)2 * MT * kSlWarps * 32 * sizeof(float4) + 2 * kSlMaxStages * sizeof(uint64_t);
+  const size_t stage = SlW<WT>::kBytes + (size_t)MT * kSlXBytes;
+  const size_t fixed = 1024 + (size_t)2 * MT * kSlWarps * 32 * sizeof(float4) + 2 * SlW<WT>::kMaxStages * sizeof(uint64_t);
   StreamPlan p;
   p.ctas_per_sm = 2;
   int s = (int)((kSlSmemTwoPerSM - fixed) / stage);
@@ -464,7 +537,7 @@ static StreamPlan stream_plan(int MT) {
     p.ctas_per_sm = 1;
     s = (int)((kSlSmemOnePerSM - fixed) / stage);
   }
-  if (s > kSlMaxStages) s = kSlMaxStages;
+  if (s > SlW<WT>::kMaxStages) s = SlW<WT>::kMaxStages;
   p.stages = s;
   p.smem = fixed + (size_t)s * stage;
   return p;
@@ -507,9 +580,9 @@ static int sl_encode(CUtensorMap* map, const void* base, int rows, int K, long l
   return TF_OK;
 }
 
-template <int MT>
+template <int MT, typename WT = __half>
 static int launch_stream(const CUtensorMap& wmap, const CUtensorMap& xmap, const StreamArgs& a, size_t smem, int grid, cudaStream_t stream) {
-  auto kern = stream_linear_kernel<MT>;
+  auto kern = stream_linear_kernel<MT, WT>;
   int dev = 0;
   TF_CHECK_CUDA(cudaGetDevice(&dev));
   static size_t configured[64] = {0};  // per device: the attribute is per (function, device)
@@ -520,6 +593,88 @@ static int launch_stream(const CUtensorMap& wmap, const CUtensorMap& xmap, const
   }
   TF_CHECK_CUDA(launch_kernel(kPdlStream, kern, dim3(grid), dim3(kSlThreads), smem, stream, wmap, xmap, a));
   TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+// ---- E4M3 weights: per-row quantization and dequantization (the rule of common.cuh with e clamped at -15) ----------------
+constexpr int kWqThreads = 256;
+constexpr uint32_t kWqRefuseAbove = 0x7b80u;  // fp16 bits of 61440 = 240 * 2^8
+
+__device__ __forceinline__ int weight_e4m3_exponent(float amax) {
+  const int e = kv_e4m3_exponent(amax);
+  return e < -15 ? -15 : e;  // code * 2^e stays an exact fp16 value (codes are multiples of 2^-9 with <= 4 significant bits)
+}
+
+// one CTA per row: max |w| over K as the largest fp16 magnitude bit pattern (NaN / inf compare above every finite value),
+// then the codes of 8 elements per thread and step
+__global__ void __launch_bounds__(kWqThreads) weight_quantize_e4m3_kernel(const __half* __restrict__ W, long long row_stride, int K,
+                                                                         uint8_t* __restrict__ codes, long long codes_row_stride,
+                                                                         int8_t* __restrict__ exps, int32_t* refused) {
+  __shared__ uint32_t red[kWqThreads / 32];
+  const int row = blockIdx.x;
+  const __half* w = W + (size_t)row * row_stride;
+  uint32_t m = 0;
+  for (int k = threadIdx.x * 8; k < K; k += kWqThreads * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(w + k);
+    const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) m = max(m, max(u[i] & 0x7fffu, (u[i] >> 16) & 0x7fffu));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = red[0];
+#pragma unroll
+  for (int i = 1; i < kWqThreads / 32; ++i) m = max(m, red[i]);
+  if (m > kWqRefuseAbove) {  // non-finite, or large enough for D to round past the fp16 maximum: counted, row left alone
+    if (threadIdx.x == 0 && refused) atomicAdd(refused, 1);
+    return;
+  }
+  const int e = weight_e4m3_exponent(__half2float(__ushort_as_half((unsigned short)m)));
+  if (threadIdx.x == 0) exps[row] = (int8_t)e;
+  uint8_t* c = codes + (size_t)row * codes_row_stride;
+  for (int k = threadIdx.x * 8; k < K; k += kWqThreads * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(w + k);
+    const __half2* h = reinterpret_cast<const __half2*>(&v);
+    uint2 o;
+    uint32_t q[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 f = __half22float2(h[i]);
+      q[i] = kv_e4m3_quantize2(f.x, f.y, e);
+    }
+    o.x = q[0] | (q[1] << 16);
+    o.y = q[2] | (q[3] << 16);
+    *reinterpret_cast<uint2*>(c + k) = o;
+  }
+}
+
+__global__ void __launch_bounds__(kWqThreads) weight_dequantize_e4m3_kernel(const uint8_t* __restrict__ codes, long long codes_row_stride,
+                                                                           const int8_t* __restrict__ exps, int K, __half* __restrict__ D,
+                                                                           long long d_row_stride) {
+  const int row = blockIdx.x;
+  const int e = exps[row];
+  const uint8_t* c = codes + (size_t)row * codes_row_stride;
+  __half* d = D + (size_t)row * d_row_stride;
+  for (int k = threadIdx.x * 8; k < K; k += kWqThreads * 8)
+    *reinterpret_cast<uint4*>(d + k) = kv_e4m3_dequant8(*reinterpret_cast<const uint2*>(c + k), e);
+}
+
+// codes [rows][row_stride bytes] seen as (32 bytes, rows, K/32), fastest first; box = 32 x 8 rows x 8 = 8 rows x 256 k, no swizzle
+static int sl_encode_e4m3(CUtensorMap* map, const void* base, int rows, int K, long long row_stride) {
+  PFN_encodeTiledSL encode = sl_encoder();
+  if (!encode) return TF_ERR_CUDA;
+  cuuint64_t gdim[3] = {32, (cuuint64_t)rows, (cuuint64_t)(K / 32)};
+  cuuint64_t gstride[2] = {(cuuint64_t)row_stride, 32};
+  cuuint32_t box[3] = {32, 8, 8};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled (e4m3 weights) failed with CUresult %d", (int)r);
+    return TF_ERR_CUDA;
+  }
   return TF_OK;
 }
 
@@ -548,7 +703,7 @@ size_t tf_stream_linear_workspace_bytes(void) {
 
 static int stream_linear_impl(const void* x, long long x_row_stride, const void* w_tensormap, int M, int N, int K, int epilogue, void* y,
                               long long y_row_stride, void* workspace, size_t workspace_bytes, const tf::StreamPeers* peers,
-                              tf_stream_t stream_) {
+                              tf_stream_t stream_, const int8_t* wexp = nullptr) {
   using namespace tf;
   TF_CHECK_ARG(x && w_tensormap && (y || epilogue == 4) && workspace, "tf_stream_linear: NULL pointer");
   TF_CHECK_ARG(workspace_bytes >= tf_stream_linear_workspace_bytes() && ((uintptr_t)workspace & 15) == 0, "tf_stream_linear: workspace too small or misaligned");
@@ -558,7 +713,7 @@ static int stream_linear_impl(const void* x, long long x_row_stride, const void*
   TF_CHECK_ARG(epilogue != 1 || (N % 2 == 0), "tf_stream_linear: the SiLU epilogue needs N = 2*inter");
   TF_CHECK_ARG(((uintptr_t)x & 15) == 0 && x_row_stride >= K && x_row_stride % 8 == 0, "tf_stream_linear: x / x_row_stride must keep 16-byte alignment");
   const int MT = (M + 7) / 8;
-  const StreamPlan plan = stream_plan(MT);
+  const StreamPlan plan = wexp ? stream_plan<__nv_fp8_e4m3>(MT) : stream_plan(MT);
   CUtensorMap wmap, xmap;
   memcpy(&wmap, w_tensormap, sizeof(wmap));
   int rc = sl_encode(&xmap, x, M, K, x_row_stride, 8, false);
@@ -567,6 +722,7 @@ static int stream_linear_impl(const void* x, long long x_row_stride, const void*
   a.M = M; a.N = N; a.K = K; a.epilogue = epilogue; a.y = y; a.y_row_stride = y_row_stride; a.stages = plan.stages;
   memset(&a.peers, 0, sizeof(a.peers));
   if (peers) a.peers = *peers;
+  a.wexp = wexp;
   const int tiles = epilogue == 1 ? (N / 2 + 7) / 8 : (N + kSlRows - 1) / kSlRows;
   int sms = sm_count();
   if (sms <= 0) sms = 132;
@@ -575,6 +731,13 @@ static int stream_linear_impl(const void* x, long long x_row_stride, const void*
   a.part = (float4*)workspace;
   a.flags = (int*)((uint8_t*)workspace + (size_t)(2 * sms + 1) * 3 * 32 * sizeof(float4));
   cudaStream_t stream = (cudaStream_t)stream_;
+  if (wexp) {
+    switch (MT) {
+      case 1: return launch_stream<1, __nv_fp8_e4m3>(wmap, xmap, a, plan.smem, grid, stream);
+      case 2: return launch_stream<2, __nv_fp8_e4m3>(wmap, xmap, a, plan.smem, grid, stream);
+      default: return launch_stream<3, __nv_fp8_e4m3>(wmap, xmap, a, plan.smem, grid, stream);
+    }
+  }
   switch (MT) {
     case 1: return launch_stream<1>(wmap, xmap, a, plan.smem, grid, stream);
     case 2: return launch_stream<2>(wmap, xmap, a, plan.smem, grid, stream);
@@ -637,6 +800,57 @@ int tf_stream_linear_ll_push(const void* x, long long x_row_stride, const void* 
   peers.epoch = const_cast<int32_t*>(epoch_and_counter);  // read only: the consumer (tf_add_rmsnorm_ll) advances it
   peers.ll_slots_per_src = cap / 4;
   return stream_linear_impl(x, x_row_stride, w_tensormap, M, N, K, 4, nullptr, 0, workspace, workspace_bytes, &peers, stream);
+}
+
+int tf_weight_quantize_e4m3(const void* W, long long row_stride, int N, int K, void* codes, long long codes_row_stride, int8_t* exps,
+                            int32_t* refused_rows, tf_stream_t stream) {
+  using namespace tf;
+  TF_CHECK_ARG(W && codes && exps, "tf_weight_quantize_e4m3: NULL pointer");
+  TF_CHECK_ARG(N >= 1 && K >= 64 && K % 64 == 0, "tf_weight_quantize_e4m3: need N >= 1 and K a positive multiple of 64 (N=%d, K=%d)", N, K);
+  TF_CHECK_ARG(((uintptr_t)W & 15) == 0 && row_stride >= K && row_stride % 8 == 0, "tf_weight_quantize_e4m3: W / row_stride must keep 16-byte alignment");
+  TF_CHECK_ARG(((uintptr_t)codes & 15) == 0 && codes_row_stride >= K && codes_row_stride % 16 == 0, "tf_weight_quantize_e4m3: codes / codes_row_stride must keep 16-byte alignment");
+  weight_quantize_e4m3_kernel<<<N, kWqThreads, 0, (cudaStream_t)stream>>>((const __half*)W, row_stride, K, (uint8_t*)codes, codes_row_stride, exps,
+                                                                         refused_rows);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_weight_dequantize_e4m3(const void* codes, long long codes_row_stride, const int8_t* exps, int N, int K, void* D, long long d_row_stride,
+                              tf_stream_t stream) {
+  using namespace tf;
+  TF_CHECK_ARG(codes && exps && D, "tf_weight_dequantize_e4m3: NULL pointer");
+  TF_CHECK_ARG(N >= 1 && K >= 64 && K % 64 == 0, "tf_weight_dequantize_e4m3: need N >= 1 and K a positive multiple of 64 (N=%d, K=%d)", N, K);
+  TF_CHECK_ARG(((uintptr_t)codes & 15) == 0 && codes_row_stride >= K && codes_row_stride % 16 == 0, "tf_weight_dequantize_e4m3: codes / codes_row_stride must keep 16-byte alignment");
+  TF_CHECK_ARG(((uintptr_t)D & 15) == 0 && d_row_stride >= K && d_row_stride % 8 == 0, "tf_weight_dequantize_e4m3: D / d_row_stride must keep 16-byte alignment");
+  weight_dequantize_e4m3_kernel<<<N, kWqThreads, 0, (cudaStream_t)stream>>>((const uint8_t*)codes, codes_row_stride, exps, K, (__half*)D, d_row_stride);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_weight_tensormap_encode_e4m3(void* out, const void* codes, int N, int K, long long row_stride) {
+  using namespace tf;
+  TF_CHECK_ARG(out && codes, "tf_weight_tensormap_encode_e4m3: NULL pointer");
+  TF_CHECK_ARG(N >= 1 && K >= 64 && K % 64 == 0, "tf_weight_tensormap_encode_e4m3: need N >= 1 and K a positive multiple of 64 (N=%d, K=%d)", N, K);
+  TF_CHECK_ARG(((uintptr_t)codes & 15) == 0 && row_stride >= K && row_stride % 16 == 0, "tf_weight_tensormap_encode_e4m3: codes / row_stride must keep 16-byte alignment");
+  CUtensorMap map;
+  int rc = sl_encode_e4m3(&map, codes, N, K, row_stride);
+  if (rc != TF_OK) return rc;
+  memcpy(out, &map, sizeof(map));
+  return TF_OK;
+}
+
+int tf_stream_linear_e4m3(const void* x, long long x_row_stride, const void* w_tensormap, const int8_t* w_exp, int M, int N, int K,
+                          int epilogue, void* y, long long y_row_stride, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  if (epilogue >= 3) {
+    tf::set_error("tf_stream_linear_e4m3: epilogue %d not in {0 fp16, 1 silu*up, 2 fp32} (no TP seams over E4M3 weights)", epilogue);
+    return TF_ERR_INVALID;
+  }
+  if (!w_exp) {
+    tf::set_error("tf_stream_linear_e4m3: NULL exponents");
+    return TF_ERR_INVALID;
+  }
+  return stream_linear_impl(x, x_row_stride, w_tensormap, M, N, K, epilogue, y, y_row_stride, workspace, workspace_bytes, nullptr, stream,
+                            w_exp);
 }
 
 }  // extern "C"

@@ -48,8 +48,10 @@ class InferenceEngine:
         (the reference's chunking, kept because it fixes the fp16 summation order the golden logits were produced with);
         the last call with exactly one id also builds the retrieval cache inside `LlamaModel.forward_target`
         (modeling_llama.py:230-238).  Up to 64 ids = a verify / decode step over the full KV (`tf_verify_attn`)."""
-        if input_ids.shape[-1] > 64 and getattr(self.kv_cache, "kv_dtype", "fp16") == "e4m3":
-            # layer-major prefill: the prompt's attention runs on an fp16 scratch layer, then the layer is quantized
+        if input_ids.shape[-1] > 64 and (getattr(self.kv_cache, "kv_dtype", "fp16") == "e4m3"
+                                         or getattr(self.model, "weight_dtype", "fp16") == "e4m3"):
+            # layer-major prefill: on an E4M3 store the prompt's attention runs on an fp16 scratch layer, then the layer is
+            # quantized; E4M3 weights are dequantized once per layer instead of once per chunk
             logits = self.model.prefill_e4m3(input_ids, self.kv_cache, chunk=self.target_prefill_chunk)
         elif input_ids.shape[-1] > 64:  # prefill
             c = self.target_prefill_chunk

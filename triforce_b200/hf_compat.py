@@ -78,9 +78,14 @@ class _Factory:
 
     @classmethod
     def from_pretrained(cls, name_or_path: str, torch_dtype=torch.float16, device_map=None, synthetic=None, seed: int = 0,
-                        config: LlamaShape = None, gqa_retrieval: Optional[str] = None, **kw) -> LlamaModel:
+                        config: LlamaShape = None, gqa_retrieval: Optional[str] = None, weight_dtype: str = "fp16", **kw) -> LlamaModel:
+        """weight_dtype="e4m3": the target's projection weights in FP8 E4M3 (see LlamaModel); the draft stays fp16."""
         if torch_dtype not in (None, torch.float16):
             raise ValueError("the TriForce hot path is fp16 (reference: torch_dtype=torch.float16)")
+        if weight_dtype not in ("fp16", "e4m3"):
+            raise ValueError(f"weight_dtype must be 'fp16' or 'e4m3', got {weight_dtype!r}")
+        if weight_dtype != "fp16" and cls.is_draft:
+            raise ValueError("the draft keeps fp16 weights (weight_dtype='e4m3' is for the target)")
         is_dir = os.path.isdir(name_or_path)
         if config is not None:
             shape = config
@@ -102,11 +107,11 @@ class _Factory:
         else:
             raise FileNotFoundError(f"{name_or_path}: not a local checkpoint directory and there is no network (HF_HUB_OFFLINE); "
                                     "pass synthetic=True or set TRIFORCE_SYNTHETIC=1 for seeded random-init weights")
-        return cls._make(shape, sd, dev)
+        return cls._make(shape, sd, dev, weight_dtype)
 
     @classmethod
-    def _make(cls, shape, sd, dev):
-        return LlamaModel(shape, sd, device=dev, is_draft=cls.is_draft)
+    def _make(cls, shape, sd, dev, weight_dtype="fp16"):
+        return LlamaModel(shape, sd, device=dev, is_draft=cls.is_draft, weight_dtype=weight_dtype)
 
 
 class TargetLlamaForCausalLM(_Factory):

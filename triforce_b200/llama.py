@@ -86,13 +86,34 @@ def shard_layer_weights(state_dict: Dict[str, torch.Tensor], config: LlamaShape,
 
 
 _PUSHED = object()  # a seam whose sum over ranks is still sitting in the LL inboxes (see LlamaModel._seam)
+WEIGHT_DTYPES = ("fp16", "e4m3")
+
+
+def require_fp16_weights(model, what: str) -> None:
+    """Paths without an E4M3-weight implementation refuse such a model instead of running on weights it does not hold."""
+    if getattr(model, "weight_dtype", "fp16") != "fp16":
+        raise NotImplementedError(f"{what} needs fp16 projection weights; this target stores them in {model.weight_dtype}")
 
 
 class LlamaModel:
     """Weights + forward of one Llama (target or draft) on one GPU (optionally one tensor-parallel shard)."""
 
     def __init__(self, config: LlamaShape, state_dict: Dict[str, torch.Tensor], device="cuda", is_draft: bool = False,
-                 tp_rank: int = 0, tp_world: int = 1, prefill_chunk: int = 128):
+                 tp_rank: int = 0, tp_world: int = 1, prefill_chunk: int = 128, weight_dtype: str = "fp16"):
+        """weight_dtype="e4m3" stores the projection weights (q|k|v, o_proj, gate|up, down_proj, lm_head) in FP8 E4M3 with one
+        power-of-two exponent per row (ops.E4m3WeightMap); embeddings and norms stay fp16.  This changes the target's numerics:
+        the model computed is the one whose weights are D = code * 2^e, exactly as an fp16 model holding D would compute it."""
+        if weight_dtype not in WEIGHT_DTYPES:
+            raise ValueError(f"weight_dtype must be one of {WEIGHT_DTYPES}, got {weight_dtype!r}")
+        if weight_dtype == "e4m3":
+            if is_draft:
+                raise ValueError("the draft keeps fp16 weights (weight_dtype='e4m3' is for the target)")
+            if tp_world > 1:
+                raise NotImplementedError("E4M3 weights are not supported under tensor parallelism (the TP seams are fp16)")
+            if os.environ.get("TRIFORCE_STREAM_LINEAR", "1") != "1":
+                raise NotImplementedError("E4M3 weights run their decode projections on tf_stream_linear_e4m3; "
+                                          "TRIFORCE_STREAM_LINEAR=0 has no E4M3 path")
+        self.weight_dtype = weight_dtype
         self.config = config
         self.device = torch.device(device)
         self.dtype = torch.float16
@@ -114,14 +135,22 @@ class LlamaModel:
         def g(name):
             return state_dict[name].to(device=self.device, dtype=torch.float16)
 
+        e4m3 = weight_dtype == "e4m3"
+        q8 = ops.E4m3WeightMap.quantize
         self.embed_tokens = g("model.embed_tokens.weight")
         self.lm_head = g("lm_head.weight")
+        self.m_lm_head = None
+        if e4m3:  # quantize each matrix as soon as it exists and keep no fp16 copy
+            self.m_lm_head, self.lm_head = q8(self.lm_head), None
         self.norm = g("model.norm.weight")
         self.layers = []
         for l in range(config.num_hidden_layers):
             p = f"model.layers.{l}."
             w = _LayerWeights()
             w.wqkv, w.wo, w.wgu, w.wd = shard_layer_weights(state_dict, config, l, tp_rank, tp_world, device=self.device)
+            if e4m3:
+                w.m_qkv, w.m_o, w.m_gu, w.m_d = q8(w.wqkv), q8(w.wo), q8(w.wgu, silu=True), q8(w.wd)
+                w.wqkv = w.wo = w.wgu = w.wd = None
             w.ln1 = g(p + "input_layernorm.weight")
             w.ln2 = g(p + "post_attention_layernorm.weight")
             self.layers.append(w)
@@ -135,8 +164,11 @@ class LlamaModel:
         self.use_stream_linear = os.environ.get("TRIFORCE_STREAM_LINEAR", "1") == "1" and self.device.type == "cuda"
         self.use_skinny_gemm = os.environ.get("TRIFORCE_SKINNY_GEMM", "1") == "1"
         self._linear_ws = None
-        self.m_lm_head = None
-        if self.use_stream_linear:
+        self._dense_buf, self._dense_of = None, None  # E4M3 weights: the one-layer fp16 scratch of > 24-row forwards
+        if e4m3:
+            self._linear_ws = torch.zeros(_C_lib().tf_stream_linear_workspace_bytes(), dtype=torch.uint8, device=self.device)
+            self._act_pad = None
+        elif self.use_stream_linear:
             self._build_weight_maps()
         self.peer_allreduce = None  # set by enable_peer_allreduce() on TP ranks
         self.peer_linear = None     # fused row-parallel linear + all-reduce (one kernel over NVLink peer memory)
@@ -172,6 +204,23 @@ class LlamaModel:
                 if self._act_pad is None:
                     self._act_pad = torch.zeros((ops.STREAM_MAX_ROWS, Kp), dtype=torch.float16, device=self.device)
         self.m_lm_head = mk(self.lm_head)
+
+    def _dense(self, which):
+        """E4M3 weights, forwards of more than 24 rows: D of layer `which` (wqkv, wo, wgu, wd) or of lm_head (`which` = "head") in a
+        one-layer fp16 scratch, dequantized only when the layer it holds changes (lm_head reuses the same memory)."""
+        maps = (self.m_lm_head,) if which == "head" else tuple(getattr(self.layers[which], n) for n in ("m_qkv", "m_o", "m_gu", "m_d"))
+        if self._dense_buf is None:
+            per_layer = sum(m.N * m.K for m in (self.layers[0].m_qkv, self.layers[0].m_o, self.layers[0].m_gu, self.layers[0].m_d))
+            self._dense_buf = torch.empty(max(per_layer, self.m_lm_head.N * self.m_lm_head.K), dtype=torch.float16, device=self.device)
+        out, off = [], 0
+        for m in maps:
+            out.append(self._dense_buf[off:off + m.N * m.K].view(m.N, m.K))
+            off += m.N * m.K
+        if self._dense_of != which:
+            for m, t in zip(maps, out):
+                ops.weight_dequantize_e4m3(m.codes, m.exps, out=t)
+            self._dense_of = which
+        return out
 
     def _tc_workspace(self, rows: int, maps) -> torch.Tensor:
         """Split-partial workspace of the wgmma attention (tf_tree_attn_tc) for `rows` query rows over this store."""
@@ -320,10 +369,14 @@ class LlamaModel:
         w = self.layers[l]
         n = h.shape[0]
         stream = self.use_stream_linear and n <= ops.STREAM_MAX_ROWS  # per projection: a shard whose K is not a multiple of 64 keeps the fallback
+        if self.weight_dtype == "e4m3" and not stream:
+            wqkv, wo, wgu, wd = self._dense(l)  # cuBLAS on D
+        else:
+            wqkv, wo, wgu, wd = w.wqkv, w.wo, w.wgu, w.wd
         self._add_norm(h, delta, w.ln1, x)
-        qkv = self._linear(x, w.wqkv, w.m_qkv if stream else None)
+        qkv = self._linear(x, wqkv, w.m_qkv if stream else None)
         attn = attn_fn(l, qkv, n)
-        o = self._seam(attn.view(n, -1), w.wo, w.m_o if stream else None)
+        o = self._seam(attn.view(n, -1), wo, w.m_o if stream else None)
         self._add_norm(h, o, w.ln2, x)
         if stream and w.m_gu is not None:
             if w.m_d is not None and w.m_d.K != self.local_inter:  # zero-padded down_proj (see _build_weight_maps)
@@ -332,17 +385,18 @@ class LlamaModel:
             else:
                 act = ops.stream_linear(x, w.m_gu, silu=True, workspace=self._linear_ws)
         else:
-            gu = self._linear(x, w.wgu)
+            gu = self._linear(x, wgu)
             act = torch.empty((n, self.local_inter), dtype=torch.float16, device=self.device)
             ops.silu_mul(gu, act)
         m_d = w.m_d if (stream and w.m_d is not None and w.m_d.K == act.shape[1]) else None
-        return self._seam(act, w.wd, m_d)
+        return self._seam(act, wd, m_d)
 
     def _head(self, h: torch.Tensor, delta, x: torch.Tensor) -> torch.Tensor:
         """Final norm + lm_head (fp32 logits) on the rows of h."""
         stream = self.use_stream_linear and h.shape[0] <= ops.STREAM_MAX_ROWS
+        lm_head = self._dense("head")[0] if (self.weight_dtype == "e4m3" and not stream) else self.lm_head
         self._add_norm(h, delta, self.norm, x)
-        return self._linear(x, self.lm_head, self.m_lm_head if stream else None, out_fp32=True)
+        return self._linear(x, lm_head, self.m_lm_head if stream else None, out_fp32=True)
 
     def _prefill_attention(self, q_out, maps, key_layer, value_layer, layer: int, kv_len: int, n: int, out, ws):
         """Causal attention of n prompt rows over an fp16 store: verify kernel up to 32 rows, wgmma at d = 128, else library."""
@@ -356,43 +410,54 @@ class LlamaModel:
         return _prefill_attention_library(q_out, key_layer, value_layer, kv_len, self.scale)
 
     def prefill_e4m3(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128) -> torch.Tensor:
-        """Prompt prefill into an E4M3 full-KV store, layer by layer, so that the prompt's causal attention never reads E4M3:
-        for each layer, every `chunk`-row piece runs through the layer with the ops and shapes of the chunk-major prefill
-        (`forward_target` on `chunk` ids at a time), appending its K/V to a one-layer fp16 scratch store with the fp16 RoPE
-        kernel and attending over it with the fp16 kernels; then the layer's rows are quantized into the E4M3 store.  The
-        residual stream of all prompt rows is kept between layers; logits are computed for the last piece only.  The logits
-        and the fp16 K/V rows are therefore bit-identical to the fp16 engine's chunk-major prefill with the same capacity."""
-        if kv_dtype_of(kv_cache) != "e4m3":
-            raise ValueError("prefill_e4m3 needs an E4M3 full-KV store")
+        """Layer-major prompt prefill, for an E4M3 full-KV store and for E4M3 weights: for each layer, every `chunk`-row piece
+        runs through the layer with the ops and shapes of the chunk-major prefill (`forward_target` on `chunk` ids at a time),
+        so each layer's weights are dequantized once rather than once per piece.  On an E4M3 store the pieces append their K/V
+        to a one-layer fp16 scratch store with the fp16 RoPE kernel and attend over it with the fp16 kernels, so the prompt's
+        causal attention never reads E4M3; then the layer's rows are quantized into the store.  On an fp16 store they append
+        into, and attend over, the store's own layer.  The residual stream of all prompt rows is kept between layers; logits are
+        computed for the last piece only.  The logits and the fp16 K/V rows are therefore bit-identical to the chunk-major
+        prefill with the same capacity and the same weights."""
+        e4m3_store = kv_dtype_of(kv_cache) == "e4m3"
         if kv_cache.seq_len != 0:
-            raise NotImplementedError("the E4M3 prefill starts from an empty full-KV store (reset the cache first)")
+            raise NotImplementedError("the layer-major prefill starts from an empty full-KV store (reset the cache first)")
         ids = input_ids.reshape(-1)
         N = ids.numel()
-        L, Hkv, cap, d = kv_cache.e4m3.shape
+        L, Hkv, cap, d = kv_cache.e4m3.shape if e4m3_store else kv_cache.key_store.shape
         if N > cap:
             raise ValueError(f"{N} prompt tokens exceed the {cap} slots of the full-KV store")
         Hl = self.local_num_heads
         h = self.embed_tokens[ids].contiguous()
         delta = [None] * ((N + chunk - 1) // chunk)
         x = torch.empty((min(chunk, N), h.shape[1]), dtype=torch.float16, device=self.device)
-        scratch_k = torch.zeros((1, Hkv, cap, d), dtype=torch.float16, device=self.device)
-        scratch_v = torch.zeros_like(scratch_k)
-        maps = ops.KVTensorMaps(scratch_k, scratch_v)
+        if e4m3_store:
+            scratch_k = torch.zeros((1, Hkv, cap, d), dtype=torch.float16, device=self.device)
+            scratch_v = torch.zeros_like(scratch_k)
+            maps = ops.KVTensorMaps(scratch_k, scratch_v)
+        else:
+            maps = kv_cache.tensor_maps
         ws = self._workspace()
         for l in range(L):
+            if e4m3_store:
+                kl, vl, ml = scratch_k[0], scratch_v[0], 0
+            else:
+                kl, vl, ml = kv_cache.key_store[l], kv_cache.value_store[l], l
             for i, c0 in enumerate(range(0, N, chunk)):
                 c1 = min(N, c0 + chunk)
 
                 def attn_fn(_l, qkv, n, c0=c0):
                     q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
                     out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-                    self._rope_append(qkv, q_out, scratch_k[0], scratch_v[0], pos0=c0, slot0=c0)
-                    return self._prefill_attention(q_out, maps, scratch_k[0], scratch_v[0], 0, c0 + n, n, out, ws)
+                    self._rope_append(qkv, q_out, kl, vl, pos0=c0, slot0=c0)
+                    return self._prefill_attention(q_out, maps, kl, vl, ml, c0 + n, n, out, ws)
 
                 delta[i] = self._layer(l, h[c0:c1], delta[i], x[:c1 - c0], attn_fn)
-            ops.kv_quantize_e4m3(scratch_k[0], kv_cache.e4m3.k_codes[l], kv_cache.e4m3.k_exp[l], 0, N)
-            ops.kv_quantize_e4m3(scratch_v[0], kv_cache.e4m3.v_codes[l], kv_cache.e4m3.v_exp[l], 0, N)
-        del scratch_k, scratch_v, maps
+            if e4m3_store:
+                ops.kv_quantize_e4m3(scratch_k[0], kv_cache.e4m3.k_codes[l], kv_cache.e4m3.k_exp[l], 0, N)
+                ops.kv_quantize_e4m3(scratch_v[0], kv_cache.e4m3.v_codes[l], kv_cache.e4m3.v_exp[l], 0, N)
+        if e4m3_store:
+            del scratch_k, scratch_v
+        del maps
         c0 = (N - 1) // chunk * chunk
         logits = self._head(h[c0:], delta[-1], x[:N - c0])
         kv_cache.seq_len = N
@@ -501,6 +566,7 @@ class LlamaModel:
                                storage_start: int) -> torch.Tensor:
         """`retrieval_tree_inference` of the reference (TP_llama_tree.py:406-425 → tensor_op.py:230-272): the n new tree nodes
         are written to retrieval slots [budget + storage_start, …) and attend to the whole budget plus their ancestors."""
+        require_fp16_weights(self, "forward_tree_retrieval (the Sequoia tree path)")
         Hl, d = self.local_num_heads, self.head_dim
         pos32 = position_ids.reshape(-1).to(torch.int32)
         T = graph_cache.tree_size
@@ -520,6 +586,7 @@ class LlamaModel:
         """The masked verify of all T tree nodes over the FULL KV (SpecTree_TP.py:168-175 → TP_llama_tree `inference` with an
         attention mask): nodes are appended at slots [seq_len, seq_len + T) and see the whole prefix plus their ancestors."""
         require_fp16_store(kv_cache, "forward_tree_verify")
+        require_fp16_weights(self, "forward_tree_verify (the Sequoia tree path)")
         Hl, d = self.local_num_heads, self.head_dim
         pos32 = position_ids.reshape(-1).to(torch.int32)
         T = input_ids.numel()

@@ -496,6 +496,74 @@ class WeightMap:
         return W.is_cuda and W.dtype == torch.float16 and int(W.shape[1]) % 64 == 0 and rows <= STREAM_MAX_ROWS
 
 
+class E4m3WeightMap:
+    """One projection matrix stored in E4M3 (the format of include/triforce_b200.h): codes uint8 [N, K], exponents int8 [N] and
+    the TMA descriptor of the codes for `stream_linear` (tf_weight_tensormap_encode_e4m3).  The matrix it stands for is
+    D = code * 2^e, exact in fp16 (`weight_dequantize_e4m3`).  silu=True: the [gate; up] stack of an MLP."""
+
+    def __init__(self, codes: torch.Tensor, exps: torch.Tensor, silu: bool = False):
+        require_cuda(codes, exps)
+        assert codes.dtype == torch.uint8 and codes.dim() == 2 and codes.is_contiguous()
+        assert exps.dtype == torch.int8 and exps.is_contiguous() and exps.shape == (codes.shape[0],)
+        self.codes, self.exps, self.silu = codes, exps, silu
+        self.N, self.K = int(codes.shape[0]), int(codes.shape[1])
+        self.buf = (ctypes.c_uint8 * 128)()
+        check(lib().tf_weight_tensormap_encode_e4m3(ctypes.addressof(self.buf), codes.data_ptr(), self.N, self.K, codes.stride(0)),
+              "tf_weight_tensormap_encode_e4m3")
+        self.ptr = ctypes.addressof(self.buf)
+
+    @staticmethod
+    def quantize(W: torch.Tensor, silu: bool = False) -> "E4m3WeightMap":
+        codes, exps = weight_quantize_e4m3(W)
+        return E4m3WeightMap(codes, exps, silu=silu)
+
+    def nbytes(self) -> int:
+        return self.codes.numel() + self.exps.numel()
+
+
+WEIGHT_E4M3_MAX = 61440.0  # 240 * 2^8: above it D = code * 2^e can round past the fp16 maximum
+
+
+def weight_quantize_e4m3(W: torch.Tensor, codes: Optional[torch.Tensor] = None, exps: Optional[torch.Tensor] = None):
+    """fp16 W [N, K] (K % 64 == 0) -> (codes uint8 [N, K], exponents int8 [N]) (tf_weight_quantize_e4m3).  Raises ValueError
+    when a row is not finite or has max|w| > WEIGHT_E4M3_MAX (synchronises the stream to read the count)."""
+    require_cuda(W)
+    _f16c(W, "W")
+    assert W.dim() == 2 and W.stride(1) == 1
+    N, K = int(W.shape[0]), int(W.shape[1])
+    if K % 64:
+        raise ValueError(f"E4M3 weights need K a multiple of 64, got K={K}")
+    if codes is None:
+        codes = torch.empty((N, K), dtype=torch.uint8, device=W.device)
+    if exps is None:
+        exps = torch.empty(N, dtype=torch.int8, device=W.device)
+    assert codes.dtype == torch.uint8 and codes.shape == (N, K) and codes.stride(1) == 1
+    assert exps.dtype == torch.int8 and exps.shape == (N,) and exps.is_contiguous()
+    refused = torch.zeros(1, dtype=torch.int32, device=W.device)
+    check(lib().tf_weight_quantize_e4m3(W.data_ptr(), W.stride(0), N, K, codes.data_ptr(), codes.stride(0), exps.data_ptr(),
+                                        refused.data_ptr(), stream_ptr()), "tf_weight_quantize_e4m3")
+    COUNTER.n += 1
+    bad = int(refused.item())
+    if bad:
+        raise ValueError(f"{bad} of {N} weight rows cannot be stored in E4M3: not finite, or max|w| > {WEIGHT_E4M3_MAX:g}")
+    return codes, exps
+
+
+def weight_dequantize_e4m3(codes: torch.Tensor, exps: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """D = code * 2^e as fp16 [N, K] (tf_weight_dequantize_e4m3); `out` may be a wider-strided view."""
+    require_cuda(codes, exps)
+    N, K = int(codes.shape[0]), int(codes.shape[1])
+    assert codes.dtype == torch.uint8 and codes.stride(1) == 1 and exps.dtype == torch.int8 and exps.shape == (N,)
+    if out is None:
+        out = torch.empty((N, K), dtype=torch.float16, device=codes.device)
+    _f16c(out, "out")
+    assert out.shape == (N, K) and out.stride(1) == 1
+    check(lib().tf_weight_dequantize_e4m3(codes.data_ptr(), codes.stride(0), exps.data_ptr(), N, K, out.data_ptr(), out.stride(0),
+                                          stream_ptr()), "tf_weight_dequantize_e4m3")
+    COUNTER.n += 1
+    return out
+
+
 STREAM_MAX_ROWS = 24
 _LINEAR_WS = {}
 
@@ -512,8 +580,10 @@ def stream_linear_workspace(device) -> torch.Tensor:
 def stream_linear(x: torch.Tensor, W, *, silu: bool = False, out_fp32: bool = False, out: Optional[torch.Tensor] = None,
                   workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
     """y = epilogue(x @ W.T) in one weight-streaming kernel (tf_stream_linear), x [M<=24, K], W a WeightMap (or a tensor,
-    encoded on the fly).  silu: W = [gate; up] and y[M, N/2] = SiLU(gate) * up.  out_fp32: y = float(fp16(x @ W.T))."""
-    if not isinstance(W, WeightMap):
+    encoded on the fly).  silu: W = [gate; up] and y[M, N/2] = SiLU(gate) * up.  out_fp32: y = float(fp16(x @ W.T)).
+    W an E4m3WeightMap: tf_stream_linear_e4m3, bit-identical to the fp16 kernel on D."""
+    e4m3 = isinstance(W, E4m3WeightMap)
+    if not e4m3 and not isinstance(W, WeightMap):
         W = WeightMap(W, silu=silu)
     assert W.silu == silu, "the WeightMap was encoded for the other epilogue"
     assert not (silu and out_fp32)
@@ -526,8 +596,13 @@ def stream_linear(x: torch.Tensor, W, *, silu: bool = False, out_fp32: bool = Fa
         out = torch.empty((M, N // 2 if silu else N), dtype=torch.float32 if out_fp32 else torch.float16, device=x.device)
     if workspace is None:
         workspace = stream_linear_workspace(x.device)
-    check(lib().tf_stream_linear(x.data_ptr(), x.stride(0), W.ptr, M, N, K, 1 if silu else (2 if out_fp32 else 0), out.data_ptr(),
-                                 out.stride(0), workspace.data_ptr(), workspace.numel(), stream_ptr()), "tf_stream_linear")
+    epilogue = 1 if silu else (2 if out_fp32 else 0)
+    if e4m3:
+        check(lib().tf_stream_linear_e4m3(x.data_ptr(), x.stride(0), W.ptr, W.exps.data_ptr(), M, N, K, epilogue, out.data_ptr(),
+                                          out.stride(0), workspace.data_ptr(), workspace.numel(), stream_ptr()), "tf_stream_linear_e4m3")
+    else:
+        check(lib().tf_stream_linear(x.data_ptr(), x.stride(0), W.ptr, M, N, K, epilogue, out.data_ptr(), out.stride(0),
+                                     workspace.data_ptr(), workspace.numel(), stream_ptr()), "tf_stream_linear")
     COUNTER.n += 1
     return out
 

@@ -100,6 +100,8 @@ class SpecTree:
     def __init__(self, engine, temperature: float = 0.6, top_p: float = 0.9, max_length=256, vocab_size=32000, grow_map=None,
                  residual_graph=None, sampling_callables=None, sample_gather_indices=None, tokenizer=None, noise=None) -> None:
         require_fp16_store(getattr(engine, "kv_cache", None), "SpecTree (the Sequoia tree path)")
+        if getattr(getattr(engine, "model", None), "weight_dtype", "fp16") != "fp16":
+            raise NotImplementedError("SpecTree (the Sequoia tree path) needs a target with fp16 projection weights")
         self.graph_engine = engine
         self.temperature, self.top_p = temperature, top_p
         self.residual_graph = residual_graph or get_residual

@@ -114,6 +114,9 @@ def retune_agreement(target, draft, alpha_t: float, alpha_d: float, state: dict)
     are.  alpha can only go down to 0 once (0 cannot be scaled back up): sweep in descending order."""
     import torch
 
+    if getattr(target, "weight_dtype", "fp16") != "fp16":
+        raise NotImplementedError("retune_agreement rescales fp16 projection weights in place; this target stores them in "
+                                  f"{target.weight_dtype}")
     hd, ht = draft.config.hidden_size, target.config.hidden_size
     with torch.no_grad():
         if not state.get("shared_table"):

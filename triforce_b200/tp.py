@@ -228,10 +228,12 @@ class DistributedLlama:
     def __init__(self, model_name_or_path: str, dtype=torch.float16, kv_offload=False, on_chip_layers=32, local_rank=0, world_size=1,
                  prefill=32768, bsz=1, gen_len=256, retrieval_budget=4096, retrieval_chunk_size=8, gamma=6, temperature=0.6,
                  top_p=0.9, ssl=0, draft=None, draft_cache=None, flash_attn=True, config: Optional[LlamaShape] = None,
-                 tree_size: int = 0, kv_dtype: str = "fp16") -> None:
+                 tree_size: int = 0, kv_dtype: str = "fp16", weight_dtype: str = "fp16") -> None:
         assert bsz == 1
         if kv_dtype != "fp16":
             raise NotImplementedError(f"DistributedLlama (tensor parallel) keeps an fp16 full-KV store; kv_dtype={kv_dtype!r} is not supported")
+        if weight_dtype != "fp16":
+            raise NotImplementedError(f"DistributedLlama (tensor parallel) keeps fp16 weights; weight_dtype={weight_dtype!r} is not supported")
         self.device = torch.device("cuda", local_rank)
         self.dtype = dtype
         self.local_rank, self.world_size = local_rank, world_size
