@@ -60,7 +60,8 @@ int tf_kv_tensormap_encode(void* out_tensormap_128B, const void* base, int d, lo
  * Row x (d fp16 values: K after RoPE, or V): e = the smallest integer with max|x| <= 448 * 2^e (0 for an all-zero row; in
  * [-32, 8] for finite fp16 x); code = e4m3_rn(x / 2^e), round to nearest even (exact division, nothing saturates).  The row
  * the store holds is D = fp16_rn(code * 2^e).  Every entry below that reads the store computes what its fp16 counterpart
- * computes on D; the retrieval cache it fills stays fp16.  Entries take Hq, Hkv (Hq == Hkv is MHA).
+ * computes on D.  The retrieval cache is fp16 unless it is itself stored in this format (the E4M3 retrieval cache below).
+ * Entries take Hq, Hkv (Hq == Hkv is MHA).
  * tf_kv_tensormap_encode_e4m3: tf_kv_tensormap_encode over a code store (box = one row of d bytes x box_keys rows,
  *   SWIZZLE_128B at d = 128, SWIZZLE_64B at d = 64); strides in bytes.
  * tf_kv_quantize_e4m3: fp16 rows [slot0, slot0 + n) of one layer (`src` [Hkv][..][d], head stride in elements, >= cap*d)
@@ -97,6 +98,35 @@ int tf_tail_update_e4m3(const void* K, const void* V, const int8_t* Kexp, const 
                         long long kv_head_stride, void* retrK, void* retrV, long long r_layer_stride, long long r_head_stride,
                         int n_layers, int H, int d, int prefill, int budget, int seq_len_host, const int32_t* seq_len_dev,
                         int max_new, tf_stream_t stream);
+
+/* ---- E4M3 retrieval cache (opt-in; fp16 stays the default) ---------------------------------------------------------
+ * The retrieval cache in the store format above: codes [L][Hkv][rcap][d] and exponents [L][Hkv][rcap] for K and for V, rcap =
+ * budget + gamma + 1 rounded up to TF_VERIFY_BOX_KEYS.  The retrieval level only proposes tokens and the full-KV verify
+ * accepts them against the target, so this format changes acceptance but not the target or the distribution of its tokens.
+ * The full store is fp16 (Kexp = Vexp = NULL, strides in elements) or E4M3 (strides in bytes); strides of both are multiples
+ * of d and the exponent strides are the code strides divided by d.  d in {64, 128}.
+ * tf_retrieval_build_to_e4m3: tf_retrieval_build_gqa / tf_retrieval_build_e4m3 (Hq == Hkv: MHA) with the gather writing the
+ *   E4M3 cache: an fp16 row is quantized by the rule above, an E4M3 row's codes and exponent are copied, so the cache holds
+ *   the store's D.  Indices and scores are bit-identical to the build into an fp16 cache.
+ * tf_tail_update_to_e4m3: tf_tail_update / tf_tail_update_e4m3 into the E4M3 cache, with the same conversion per row.
+ * tf_verify_attn_e4m3_clean: tf_verify_attn_e4m3 with the `clean_keys` of tf_verify_attn: on a programmatic launch (PDL bit 16,
+ *   stores below 16 384 keys) with a host-side length, the producer loads the code tiles and exponents of keys
+ *   [0, clean_keys), which the preceding kernel must not write, before it waits on that kernel.  clean_keys = 0 is
+ *   tf_verify_attn_e4m3.
+ */
+int tf_retrieval_build_to_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                               long long kv_head_stride, const void* q, int n_layers, int Hq, int Hkv, int d, int prefill, int chunk,
+                               int budget, void* retrK, void* retrV, int8_t* retrKexp, int8_t* retrVexp, long long r_layer_stride,
+                               long long r_head_stride, int32_t* out_idx, void* out_scores, void* workspace, size_t workspace_bytes,
+                               tf_stream_t stream);
+int tf_tail_update_to_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                           long long kv_head_stride, void* retrK, void* retrV, int8_t* retrKexp, int8_t* retrVexp,
+                           long long r_layer_stride, long long r_head_stride, int n_layers, int H, int d, int prefill, int budget,
+                           int seq_len_host, const int32_t* seq_len_dev, int max_new, tf_stream_t stream);
+int tf_verify_attn_e4m3_clean(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                              long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max, int R, int Hq,
+                              int Hkv, int d, float scale, void* out, void* workspace, size_t workspace_bytes, int clean_keys,
+                              tf_stream_t stream);
 
 /* ---- (i) retrieval-cache build ---------------------------------------------------------------------------------
  * replaces models/cache.py:154-175 (RetrievalCache.init_graph_cache: ATen mean + cuBLAS bmm + ATen topk + 2 gathers;

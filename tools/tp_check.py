@@ -33,6 +33,7 @@ def main():
     ap.add_argument("--device_loop", type=int, default=0, metavar="SEED",
                     help="instead of replaying the golden trace: run the whole-loop graph (DeviceLoopRun, what bench.py times at every N) and the "
                          "step-wise loop on the same device Philox stream, each on a freshly built sharded engine, and compare their tokens")
+    ap.add_argument("--retrieval_dtype", default="fp16", choices=["fp16", "e4m3"], help="the rank-local retrieval cache's format")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -50,7 +51,7 @@ def main():
         dcache = StreamingLLMEvictionCache(draft, start_size=16, recent_size=256 - 16 - gamma, gamma=gamma)
         m = DistributedLlama(case["target"], local_rank=rank, world_size=world, prefill=P, gen_len=args.gen + 16, retrieval_budget=B,
                              retrieval_chunk_size=case["chunk"], gamma=gamma, temperature=case["temperature"], top_p=case["top_p"],
-                             draft=draft, draft_cache=dcache, config=ts)
+                             draft=draft, draft_cache=dcache, config=ts, retrieval_dtype=args.retrieval_dtype)
         m.init_parameters(state_dict=numpy_state_dict(ts, case["target_seed"]))
         m.graph_engine.engine.draft_prefill_chunk = args.draft_chunk
         return m

@@ -36,6 +36,14 @@ _SIGNATURES = {
                                         c_void_p, c_size_t, c_void_p]),
     "tf_tail_update_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_longlong,
                                     c_longlong, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "tf_retrieval_build_to_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int,
+                                           c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong,
+                                           c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tf_tail_update_to_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_longlong, c_longlong, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                       c_void_p]),
+    "tf_verify_attn_e4m3_clean": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_void_p, c_int,
+                                          c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "tf_retrieval_build_workspace_bytes": (c_size_t, [c_int] * 6),
     "tf_retrieval_build": (c_int, [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                    c_int, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p,

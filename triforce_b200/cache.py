@@ -70,6 +70,11 @@ def kv_dtype_of(cache) -> str:
     return getattr(cache, "kv_dtype", "fp16")
 
 
+def _full_store_of(kv_cache):
+    """The full-KV store as the E4M3 retrieval-cache entries take it: an E4m3Store, or the fp16 (key_store, value_store) pair."""
+    return kv_cache.e4m3 if kv_dtype_of(kv_cache) == "e4m3" else (kv_cache.key_store, kv_cache.value_store)
+
+
 def require_fp16_store(cache, what: str) -> None:
     if kv_dtype_of(cache) != "fp16":
         raise NotImplementedError(f"{what} needs an fp16 full-KV store; this one is {kv_dtype_of(cache)}")
@@ -148,9 +153,17 @@ class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
 
 class RetrievalCache(_HeadMajorStore):
     """Retrieval ("graph") cache (reference cache.py:117-198): `max_budget` slots filled with the top-k chunks of the
-    full KV, followed by gamma+1 slots for the tokens being verified."""
+    full KV, followed by gamma+1 slots for the tokens being verified.
 
-    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, gamma=6) -> None:
+    kv_dtype="e4m3" stores it in the E4M3 format of the full-KV store (include/triforce_b200.h): `e4m3` holds codes and
+    exponents, `key_store` / `value_store` are the uint8 codes and the slot count is rounded up to a multiple of 64.  The
+    build and tail copy quantize the rows of an fp16 full store, or copy the codes of an E4M3 one.  The retrieval level only
+    proposes tokens, so this changes acceptance but not the target: TriForce stays lossless with respect to the full model."""
+
+    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, gamma=6, kv_dtype: str = "fp16") -> None:
+        if kv_dtype not in KV_DTYPES:
+            raise ValueError(f"kv_dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
+        self.kv_dtype = kv_dtype
         self.chunk_size = chunk_size
         self.prefill = prefill
         self.chunks = prefill // self.chunk_size
@@ -162,7 +175,15 @@ class RetrievalCache(_HeadMajorStore):
         self.real_budget = max_budget + gamma + 1
         L, H, d = _model_geometry(model)
         self.hidden_size = model.config.hidden_size
-        self._alloc(L, H, self.real_budget, d, model.device)
+        self.e4m3: Optional[ops.E4m3Store] = None
+        if kv_dtype == "e4m3":
+            slots = -(-self.real_budget // ops.VERIFY_BOX_KEYS) * ops.VERIFY_BOX_KEYS
+            self.e4m3 = ops.E4m3Store.empty(L, H, slots, d, model.device)
+            self.key_store, self.value_store = self.e4m3.k_codes, self.e4m3.v_codes
+            self.layers, self.num_heads, self.head_dim, self.slots = L, H, d, slots
+            self._maps = self.e4m3
+        else:
+            self._alloc(L, H, self.real_budget, d, model.device)
         self.init_graph = False
         # last build's selection, kept for inspection / parity tests: int32 [L, H, select_sets], fp16 [L, H, chunks]
         self.topk_idx = torch.zeros((L, H, self.select_sets), dtype=torch.int32, device=model.device)
@@ -182,6 +203,9 @@ class RetrievalCache(_HeadMajorStore):
 
     def _build(self, kv_cache: FlashSimpleCache, q: torch.Tensor, layer0: int, n: int):
         out = dict(layer0=layer0, n_layers=n, out_idx=self.topk_idx[layer0:layer0 + n], out_scores=self.chunk_scores[layer0:layer0 + n])
+        if self.e4m3 is not None:  # into the E4M3 cache, from either store (MHA, or GQA under the "group_sum" rule)
+            ops.retrieval_build_to_e4m3(_full_store_of(kv_cache), q, self.e4m3, self.prefill, self.chunk_size, self.max_budget, **out)
+            return
         if kv_dtype_of(kv_cache) == "e4m3":  # MHA, or GQA under the "group_sum" rule, over the E4M3 store
             ops.retrieval_build_e4m3(kv_cache.e4m3, q, self.key_store, self.value_store, self.prefill, self.chunk_size,
                                      self.max_budget, **out)
@@ -199,6 +223,13 @@ class RetrievalCache(_HeadMajorStore):
 
     def update_graph_cache(self, kv_cache: Optional[FlashSimpleCache] = None, use_device_len: bool = False, max_new: int = 0):
         """cache.py:180-182: KV of every committed generated token overwrites the budget tail, all layers."""
+        if self.e4m3 is not None:
+            if use_device_len:
+                ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, 0, kv_cache.seq_len_dev,
+                                        max_new)
+            else:
+                ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, kv_cache.seq_len)
+            return
         if kv_dtype_of(kv_cache) == "e4m3":  # the dequantized rows of the E4M3 store
             if use_device_len:
                 ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, 0,
@@ -215,6 +246,8 @@ class RetrievalCache(_HeadMajorStore):
 
     def update(self, new_k_cache: torch.Tensor, new_v_cache: torch.Tensor, layer_idx: int):
         """Reference-compatible spec-slot write (cache.py:184-189); the engine writes them through the RoPE kernel."""
+        if self.e4m3 is not None:
+            raise NotImplementedError("RetrievalCache.update writes fp16 rows; an e4m3 retrieval cache is written by rope_append_e4m3")
         self.key_cache[layer_idx][:, self.real_budget - self.gamma - 1:] = new_k_cache
         self.value_cache[layer_idx][:, self.real_budget - self.gamma - 1:] = new_v_cache
         return self.key_cache[layer_idx][:, :self.real_budget], self.value_cache[layer_idx][:, :self.real_budget]
@@ -223,24 +256,40 @@ class RetrievalCache(_HeadMajorStore):
         """cache.py:191-194: rebuild + per-layer tail copy (taken from the 2nd prompt on, because `reset` leaves
         `init_graph` set)."""
         self.init_graph_cache(kv_cache, query_states, layer_idx)
-        n = kv_cache.seq_len - self.prefill
-        if n > 0 and kv_dtype_of(kv_cache) == "e4m3":
-            ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, kv_cache.seq_len,
+        self.copy_tail_layer(kv_cache, kv_cache.seq_len, layer_idx)
+
+    def copy_tail_layer(self, kv_cache, seq_len: int, layer_idx: int):
+        """The per-layer tail copy of a rebuild (cache.py:191-194): full-KV rows [prefill, seq_len) of one layer go to the
+        budget tail."""
+        n = seq_len - self.prefill
+        if n <= 0:
+            return
+        if self.e4m3 is not None:
+            ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, seq_len, layer0=layer_idx,
+                                    n_layers=1)
+        elif kv_dtype_of(kv_cache) == "e4m3":
+            ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, seq_len,
                                  layer0=layer_idx, n_layers=1)
-        elif n > 0:
-            self.key_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.key_store[layer_idx, :, self.prefill:kv_cache.seq_len]
-            self.value_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.value_store[layer_idx, :, self.prefill:kv_cache.seq_len]
+        else:
+            self.key_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.key_store[layer_idx, :, self.prefill:seq_len]
+            self.value_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.value_store[layer_idx, :, self.prefill:seq_len]
 
     def reset(self):  # NB: like the reference, does not clear `init_graph`
         self.key_store.zero_()
         self.value_store.zero_()
+        if self.e4m3 is not None:
+            self.e4m3.k_exp.zero_()
+            self.e4m3.v_exp.zero_()
 
 
 class RetrievalCacheSeqouia(RetrievalCache):
     """DistributedRetrievalCache_Seqouia (reference cache.py:385-483): the retrieval budget followed by `tree_size` slots
     for the nodes of the speculation tree (instead of gamma+1 slots)."""
 
-    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, tree_size=128) -> None:
+    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, tree_size=128, kv_dtype: str = "fp16") -> None:
+        if kv_dtype != "fp16":
+            raise NotImplementedError(f"the Sequoia tree path keeps an fp16 retrieval cache (its tree growth needs a tree mode the "
+                                      f"e4m3 verify attention does not have); kv_dtype={kv_dtype!r} is not supported")
         super().__init__(model, max_budget=max_budget, prefill=prefill, chunk_size=chunk_size, gamma=tree_size - 1)
         self.tree_size = tree_size
         assert self.real_budget == max_budget + tree_size

@@ -33,6 +33,10 @@ _COMMON_TP_FLAGS = [
     ("--file", dict(type=str, default="")),
     ("--seed", dict(type=int, default=1, help="seed")),
 ]
+# addition (not in the reference) of on_chip and offloading_TP; the Sequoia tree path keeps an fp16 retrieval cache
+_RETRIEVAL_DTYPE_FLAG = ("--retrieval_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
+                                                   help="retrieval cache: fp16, or FP8 E4M3 with a per-row power-of-two scale "
+                                                        "(changes acceptance, not the target's numerics)"))
 FLAGS = {
     "on_chip": [
         ("--target", dict(type=str, default="llama-7B-128K", help="target model")),
@@ -56,8 +60,9 @@ FLAGS = {
         ("--weight_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
                                 help="target projection weights: fp16, or FP8 E4M3 with a per-row power-of-two scale "
                                      "(changes the target's numerics)")),
+        _RETRIEVAL_DTYPE_FLAG,
     ],
-    "offloading_TP": _COMMON_TP_FLAGS + [("--gamma", dict(type=str, default=6))],
+    "offloading_TP": _COMMON_TP_FLAGS + [("--gamma", dict(type=str, default=6)), _RETRIEVAL_DTYPE_FLAG],
     "offloading_seqouia": _COMMON_TP_FLAGS + [("--tree_size", dict(type=str, default="512"))],
 }
 
@@ -134,7 +139,8 @@ def run_on_chip(argv: Optional[List[str]] = None) -> None:
 
     # caches and engine (on_chip.py:76-83)
     cache = FlashSimpleCache(target, prefill + gen_len + 16, kv_dtype=args.kv_dtype)
-    graph_cache = RetrievalCache(target, max_budget=args.budget, prefill=prefill, gamma=gamma, chunk_size=args.chunk_size)
+    graph_cache = RetrievalCache(target, max_budget=args.budget, prefill=prefill, gamma=gamma, chunk_size=args.chunk_size,
+                                 kv_dtype=args.retrieval_dtype)
     draft_cache = StreamingLLMEvictionCache(draft, start_size=16, recent_size=args.draft_cache_budget - 16 - gamma, gamma=gamma)
     engine = GraphInferenceEngine(target, cache, graph_cache, draft, draft_cache)
     engine.initialize_cuda_graph(gamma, probs=True, temperature=temperature, top_p=top_p)
@@ -220,7 +226,7 @@ def run_offloading_tp(argv: Optional[List[str]] = None) -> None:
     llm = DistributedLlama(model_name_or_path=hub, local_rank=local_rank, world_size=world_size, prefill=args.prefill,
                            gen_len=args.gen_len, temperature=args.temp, top_p=args.top_p, flash_attn=True,
                            retrieval_budget=args.budget, kv_offload=True, on_chip_layers=args.on_chip, draft=draft,
-                           draft_cache=draft_cache, gamma=gamma)
+                           draft_cache=draft_cache, gamma=gamma, retrieval_dtype=args.retrieval_dtype)
     llm.init_parameters(state_dict=cuda_state_dict(llm.config, seed=1, device=device))
     tokens, latencies = [], []
     for ids in prompts:

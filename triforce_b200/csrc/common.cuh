@@ -190,5 +190,43 @@ __device__ __forceinline__ uint4 kv_e4m3_dequant8(uint2 c, int e) {
   o[3] = kv_e4m3_dequant2((uint16_t)(c.y >> 16), e);
   return r;
 }
+// one warp stores one row of D fp16 values as codes and an exponent (lane i holds elements [i*D/32, (i+1)*D/32))
+template <int D>
+__device__ __forceinline__ void kv_e4m3_quantize_row_warp(const __half* __restrict__ src, uint8_t* __restrict__ codes,
+                                                          int8_t* __restrict__ exp, int lane) {
+  constexpr int EPL = D / 32;  // elements per lane
+  const __half2* x = reinterpret_cast<const __half2*>(src + lane * EPL);
+  __half2 v[EPL / 2];
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < EPL / 2; ++i) {
+    v[i] = x[i];
+    const __half2 a = __habs2(v[i]);
+    m = fmaxf(m, fmaxf(__low2float(a), __high2float(a)));
+  }
+  const int e = kv_e4m3_exponent(warp_max(m));
+  uint16_t* out = reinterpret_cast<uint16_t*>(codes + lane * EPL);
+#pragma unroll
+  for (int i = 0; i < EPL / 2; ++i) {
+    const float2 f = __half22float2(v[i]);
+    out[i] = kv_e4m3_quantize2(f.x, f.y, e);
+  }
+  if (lane == 0) *exp = (int8_t)e;
+}
+// one warp writes row `src_row` of a full-KV store into row `dst_row` of an E4M3 store (rows index the exponents; codes and fp16
+// elements start at row * D): an fp16 source row is quantized, an E4M3 source row's codes and exponent are copied as they are
+template <int D, bool SRC_E4M3>
+__device__ __forceinline__ void kv_e4m3_row_into(const void* __restrict__ src, const int8_t* __restrict__ src_exp, size_t src_row,
+                                                 uint8_t* __restrict__ dst, int8_t* __restrict__ dst_exp, size_t dst_row, int lane) {
+  if constexpr (SRC_E4M3) {
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(src) + src_row * D;
+    uint8_t* t = dst + dst_row * D;
+    if constexpr (D == 128) reinterpret_cast<uint32_t*>(t)[lane] = reinterpret_cast<const uint32_t*>(s)[lane];
+    else reinterpret_cast<uint16_t*>(t)[lane] = reinterpret_cast<const uint16_t*>(s)[lane];
+    if (lane == 0) dst_exp[dst_row] = src_exp[src_row];
+  } else {
+    kv_e4m3_quantize_row_warp<D>(reinterpret_cast<const __half*>(src) + src_row * D, dst + dst_row * D, dst_exp + dst_row, lane);
+  }
+}
 
 }  // namespace tf

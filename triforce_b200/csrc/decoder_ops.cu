@@ -90,27 +90,11 @@ __global__ void __launch_bounds__(D / 4) rope_append_kernel(const __half* __rest
 template <int D>
 __global__ void __launch_bounds__(128) kv_quantize_kernel(const __half* __restrict__ src, long long src_head_stride, int slot0, int n,
                                                           uint8_t* __restrict__ codes, int8_t* __restrict__ exps, long long cap) {
-  constexpr int EPL = D / 32;  // elements per lane
   const int r = blockIdx.x * 4 + (threadIdx.x >> 5), h = blockIdx.y, lane = threadIdx.x & 31;
   if (r >= n) return;
   const size_t slot = (size_t)slot0 + r;
-  const __half2* x = reinterpret_cast<const __half2*>(src + (size_t)h * src_head_stride + slot * D + lane * EPL);
-  __half2 v[EPL / 2];
-  float m = 0.f;
-#pragma unroll
-  for (int i = 0; i < EPL / 2; ++i) {
-    v[i] = x[i];
-    const __half2 a = __habs2(v[i]);
-    m = fmaxf(m, fmaxf(__low2float(a), __high2float(a)));
-  }
-  const int e = kv_e4m3_exponent(warp_max(m));
-  uint16_t* out = reinterpret_cast<uint16_t*>(codes + ((size_t)h * cap + slot) * D + lane * EPL);
-#pragma unroll
-  for (int i = 0; i < EPL / 2; ++i) {
-    const float2 f = __half22float2(v[i]);
-    out[i] = kv_e4m3_quantize2(f.x, f.y, e);
-  }
-  if (lane == 0) exps[(size_t)h * cap + slot] = (int8_t)e;
+  kv_e4m3_quantize_row_warp<D>(src + (size_t)h * src_head_stride + slot * D, codes + ((size_t)h * cap + slot) * D,
+                               exps + (size_t)h * cap + slot, lane);
 }
 
 // ---- (ii) draft attention --------------------------------------------------------------------------------------------
@@ -266,6 +250,26 @@ __global__ void __launch_bounds__(256) tail_update_e4m3_kernel(const uint8_t* __
     const size_t ex = head / D + slot;
     *reinterpret_cast<uint4*>(rK + dst0 + (size_t)i * 8) = kv_e4m3_dequant8(*reinterpret_cast<const uint2*>(K + src), Ke[ex]);
     *reinterpret_cast<uint4*>(rV + dst0 + (size_t)i * 8) = kv_e4m3_dequant8(*reinterpret_cast<const uint2*>(V + src), Ve[ex]);
+  }
+}
+
+// tail_update_kernel into an E4M3 retrieval cache (tf_tail_update_to_e4m3): one warp per row, quantized from an fp16 store or
+// copied from an E4M3 one (rows index exponents; strides are multiples of D)
+template <int D, bool SRC_E4M3>
+__global__ void __launch_bounds__(256) tail_update_to_e4m3_kernel(const void* __restrict__ K, const void* __restrict__ V,
+                                                                  const int8_t* __restrict__ Ke, const int8_t* __restrict__ Ve,
+                                                                  long long kls, long long khs, uint8_t* __restrict__ rK,
+                                                                  uint8_t* __restrict__ rV, int8_t* __restrict__ rKe,
+                                                                  int8_t* __restrict__ rVe, long long rls, long long rhs, int prefill,
+                                                                  int budget, int seq_len_host, const int32_t* __restrict__ seq_len_dev) {
+  const int h = blockIdx.y, layer = blockIdx.z, lane = threadIdx.x & 31;
+  const int n_new = seq_len_host + (seq_len_dev ? *seq_len_dev : 0) - prefill;
+  if (n_new <= 0) return;
+  const size_t src0 = ((size_t)layer * kls + (size_t)h * khs) / D + prefill;
+  const size_t dst0 = ((size_t)layer * rls + (size_t)h * rhs) / D + (budget - n_new);
+  for (int r = blockIdx.x * 8 + (threadIdx.x >> 5); r < n_new; r += gridDim.x * 8) {
+    kv_e4m3_row_into<D, SRC_E4M3>(K, Ke, src0 + r, rK, rKe, dst0 + r, lane);
+    kv_e4m3_row_into<D, SRC_E4M3>(V, Ve, src0 + r, rV, rVe, dst0 + r, lane);
   }
 }
 
@@ -537,6 +541,42 @@ int tf_tail_update_e4m3(const void* K, const void* V, const int8_t* Kexp, const 
   tail_update_e4m3_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>((const uint8_t*)K, (const uint8_t*)V, Kexp, Vexp, kv_layer_stride,
                                                                    kv_head_stride, (__half*)retrK, (__half*)retrV, r_layer_stride,
                                                                    r_head_stride, d, prefill, budget, seq_len_host, seq_len_dev);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_tail_update_to_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                           long long kv_head_stride, void* retrK, void* retrV, int8_t* retrKexp, int8_t* retrVexp,
+                           long long r_layer_stride, long long r_head_stride, int n_layers, int H, int d, int prefill, int budget,
+                           int seq_len_host, const int32_t* seq_len_dev, int max_new, tf_stream_t stream_) {
+  using namespace tf;
+  TF_CHECK_ARG(K && V && retrK && retrV && retrKexp && retrVexp, "tf_tail_update_to_e4m3: NULL pointer");
+  TF_CHECK_ARG(!Kexp == !Vexp, "tf_tail_update_to_e4m3: the source's exponents are both NULL (fp16 store) or both set");
+  TF_CHECK_ARG(n_layers >= 1 && H >= 1, "tf_tail_update_to_e4m3: bad extents");
+  TF_CHECK_SUPPORTED(d == 64 || d == 128, "tf_tail_update_to_e4m3: head_dim %d not in {64,128}", d);
+  TF_CHECK_ARG(kv_layer_stride % d == 0 && kv_head_stride % d == 0 && r_layer_stride % d == 0 && r_head_stride % d == 0,
+               "tf_tail_update_to_e4m3: strides must be multiples of d");
+  TF_CHECK_ARG(((((uintptr_t)K | (uintptr_t)V | (uintptr_t)retrK | (uintptr_t)retrV)) & 7) == 0,
+               "tf_tail_update_to_e4m3: stores must be 8-byte aligned");
+  TF_CHECK_ARG(max_new >= 0 && max_new <= budget, "tf_tail_update_to_e4m3: max_new %d exceeds budget %d", max_new, budget);
+  if (!seq_len_dev) {
+    TF_CHECK_ARG(seq_len_host - prefill <= budget, "tf_tail_update_to_e4m3: %d new tokens exceed budget %d", seq_len_host - prefill,
+                 budget);
+    if (seq_len_host <= prefill) return TF_OK;
+    max_new = seq_len_host - prefill;
+  }
+  if (max_new == 0) return TF_OK;
+  int gx = (max_new + 7) / 8;  // 8 warps per CTA, one row each
+  if (gx > 16) gx = 16;
+  dim3 grid(gx, H, n_layers);
+  cudaStream_t stream = (cudaStream_t)stream_;
+#define LAUNCH_TAIL8(D_, E_)                                                                                                      \
+  tail_update_to_e4m3_kernel<D_, E_><<<grid, 256, 0, stream>>>(K, V, Kexp, Vexp, kv_layer_stride, kv_head_stride, (uint8_t*)retrK, \
+                                                               (uint8_t*)retrV, retrKexp, retrVexp, r_layer_stride, r_head_stride,  \
+                                                               prefill, budget, seq_len_host, seq_len_dev)
+  if (d == 128) { if (Kexp) LAUNCH_TAIL8(128, true); else LAUNCH_TAIL8(128, false); }
+  else { if (Kexp) LAUNCH_TAIL8(64, true); else LAUNCH_TAIL8(64, false); }
+#undef LAUNCH_TAIL8
   TF_CHECK_LAUNCH();
   return TF_OK;
 }

@@ -8,6 +8,8 @@
 // the score's query is q̄ = fp64 sum of the grp query heads of the group (exact for grp <= 64 fp16 values); grp = 1 is MHA.
 // E4M3 store (tf_retrieval_build_e4m3, the format of common.cuh): scores and gather read the codes and exponents, and every
 // K or V value they use is D, so results are those of the fp16 build on D; the gather writes D into the fp16 retrieval cache.
+// E4M3 retrieval cache (tf_retrieval_build_to_e4m3, from either store): scores and top-k are the builds above; the gather
+// quantizes each fp16 row by the store rule, or copies an E4M3 row's codes and exponent, so the cache holds the store's D.
 // All three kernels are HBM/latency bound integer+fp work; no tensor cores (task statement ①).
 #include "common.cuh"
 
@@ -210,6 +212,28 @@ __global__ void __launch_bounds__(256) gather_kernel(const void* __restrict__ K,
   }
 }
 
+// kernel 3 into an E4M3 retrieval cache (tf_retrieval_build_to_e4m3): one warp per retrieval row.  Rows index exponents; the
+// strides (in elements of the source, bytes of the cache) are multiples of D.
+template <int D, bool SRC_E4M3>
+__global__ void __launch_bounds__(256) gather_to_e4m3_kernel(const void* __restrict__ K, const void* __restrict__ V,
+                                                             const int8_t* __restrict__ Ke, const int8_t* __restrict__ Ve,
+                                                             long long kv_layer_stride, long long kv_head_stride,
+                                                             uint8_t* __restrict__ rK, uint8_t* __restrict__ rV,
+                                                             int8_t* __restrict__ rKe, int8_t* __restrict__ rVe,
+                                                             long long r_layer_stride, long long r_head_stride,
+                                                             const int32_t* __restrict__ idx, int H, int select_sets, int chunk) {
+  const int h = blockIdx.y, layer = blockIdx.z, lane = threadIdx.x & 31;
+  const int32_t* id = idx + ((size_t)layer * H + h) * select_sets;
+  const size_t src0 = ((size_t)layer * kv_layer_stride + (size_t)h * kv_head_stride) / D;
+  const size_t dst0 = ((size_t)layer * r_layer_stride + (size_t)h * r_head_stride) / D;
+  const int rows = select_sets * chunk;
+  for (int r = blockIdx.x * 8 + (threadIdx.x >> 5); r < rows; r += gridDim.x * 8) {
+    const size_t s = src0 + (size_t)id[r / chunk] * chunk + r % chunk;
+    kv_e4m3_row_into<D, SRC_E4M3>(K, Ke, s, rK, rKe, dst0 + r, lane);
+    kv_e4m3_row_into<D, SRC_E4M3>(V, Ve, s, rV, rVe, dst0 + r, lane);
+  }
+}
+
 static int next_pow2(int x) {
   int p = 1;
   while (p < x) p <<= 1;
@@ -226,7 +250,7 @@ static int retrieval_build_impl(const void* K, const void* V, long long kv_layer
                                 int n_layers, int H, int grp, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
                                 long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
                                 void* workspace, size_t workspace_bytes, tf_stream_t stream_, const int8_t* Ke = nullptr,
-                                const int8_t* Ve = nullptr);
+                                const int8_t* Ve = nullptr, int8_t* rKe = nullptr, int8_t* rVe = nullptr);
 
 size_t tf_retrieval_build_workspace_bytes(int n_layers, int H, int d, int prefill, int chunk, int budget) {
   if (n_layers <= 0 || H <= 0 || chunk <= 0) return 0;
@@ -263,6 +287,28 @@ int tf_retrieval_build_e4m3(const void* K, const void* V, const int8_t* Kexp, co
                               retrV, r_layer_stride, r_head_stride, out_idx, out_scores, workspace, workspace_bytes, stream, Kexp, Vexp);
 }
 
+int tf_retrieval_build_to_e4m3(const void* K, const void* V, const int8_t* Kexp, const int8_t* Vexp, long long kv_layer_stride,
+                               long long kv_head_stride, const void* q, int n_layers, int Hq, int Hkv, int d, int prefill, int chunk,
+                               int budget, void* retrK, void* retrV, int8_t* retrKexp, int8_t* retrVexp, long long r_layer_stride,
+                               long long r_head_stride, int32_t* out_idx, void* out_scores, void* workspace, size_t workspace_bytes,
+                               tf_stream_t stream) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0 || Hq / Hkv > 64) {
+    tf::set_error("tf_retrieval_build_to_e4m3: Hq (%d) must be a multiple of Hkv (%d), at most 64 per KV head", Hq, Hkv);
+    return TF_ERR_INVALID;
+  }
+  if (!Kexp != !Vexp || !retrKexp || !retrVexp) {
+    tf::set_error("tf_retrieval_build_to_e4m3: NULL exponent pointer (the source's are both NULL for an fp16 store, or both set)");
+    return TF_ERR_INVALID;
+  }
+  if (d <= 0 || kv_layer_stride % d != 0 || kv_head_stride % d != 0 || r_layer_stride % d != 0 || r_head_stride % d != 0) {
+    tf::set_error("tf_retrieval_build_to_e4m3: strides must be multiples of d");
+    return TF_ERR_INVALID;
+  }
+  return retrieval_build_impl(K, V, kv_layer_stride, kv_head_stride, q, n_layers, Hkv, Hq / Hkv, d, prefill, chunk, budget, retrK,
+                              retrV, r_layer_stride, r_head_stride, out_idx, out_scores, workspace, workspace_bytes, stream, Kexp, Vexp,
+                              retrKexp, retrVexp);
+}
+
 int tf_retrieval_build_gqa(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
                            int n_layers, int Hq, int Hkv, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
                            long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
@@ -278,9 +324,10 @@ int tf_retrieval_build_gqa(const void* K, const void* V, long long kv_layer_stri
 static int retrieval_build_impl(const void* K, const void* V, long long kv_layer_stride, long long kv_head_stride, const void* q,
                                 int n_layers, int H, int grp, int d, int prefill, int chunk, int budget, void* retrK, void* retrV,
                                 long long r_layer_stride, long long r_head_stride, int32_t* out_idx, void* out_scores,
-                                void* workspace, size_t workspace_bytes, tf_stream_t stream_, const int8_t* Ke, const int8_t* Ve) {
+                                void* workspace, size_t workspace_bytes, tf_stream_t stream_, const int8_t* Ke, const int8_t* Ve,
+                                int8_t* rKe, int8_t* rVe) {
   using namespace tf;
-  const bool e4m3 = Ke != nullptr;
+  const bool e4m3 = Ke != nullptr, to_e4m3 = rKe != nullptr;
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(K && V && q && retrK && retrV, "tf_retrieval_build: NULL pointer");
   TF_CHECK_ARG(n_layers > 0 && H > 0 && chunk > 0, "tf_retrieval_build: bad extents");
@@ -288,6 +335,7 @@ static int retrieval_build_impl(const void* K, const void* V, long long kv_layer
   TF_CHECK_ARG(budget % chunk == 0, "max_budget should be multiple of chunk_size, got %d %% %d", budget, chunk);
   TF_CHECK_SUPPORTED(d == 64 || d == 128 || d == 256, "tf_retrieval_build: head_dim %d not in {64,128,256}", d);
   TF_CHECK_SUPPORTED(!e4m3 || d != 256, "tf_retrieval_build_e4m3: head_dim %d not in {64,128}", d);
+  TF_CHECK_SUPPORTED(!to_e4m3 || d != 256, "tf_retrieval_build_to_e4m3: head_dim %d not in {64,128}", d);
   const int chunks = prefill / chunk, sel = budget / chunk;
   TF_CHECK_ARG(sel >= 1 && sel - 1 <= chunks - 1, "selected index k out of range (k=%d, candidates=%d)", sel - 1, chunks - 1);
   TF_CHECK_ARG(((uintptr_t)K & 15) == 0 && ((uintptr_t)V & 15) == 0 && ((uintptr_t)retrK & 15) == 0 &&
@@ -341,7 +389,16 @@ static int retrieval_build_impl(const void* K, const void* V, long long kv_layer
     int gx = (total_vec + 255) / 256;
     if (gx > 64) gx = 64;
     dim3 grid(gx, H, n_layers);
-    if (e4m3)
+    if (to_e4m3) {
+      const int rows = sel * chunk;
+      dim3 g8((rows + 7) / 8 < 64 ? (rows + 7) / 8 : 64, H, n_layers);  // 8 warps per CTA, one row each
+#define LAUNCH_GATHER8(D_, E_)                                                                                                   \
+  gather_to_e4m3_kernel<D_, E_><<<g8, 256, 0, stream>>>(K, V, Ke, Ve, kv_layer_stride, kv_head_stride, (uint8_t*)retrK,          \
+                                                        (uint8_t*)retrV, rKe, rVe, r_layer_stride, r_head_stride, idx, H, sel, chunk)
+      if (d == 128) { if (e4m3) LAUNCH_GATHER8(128, true); else LAUNCH_GATHER8(128, false); }
+      else { if (e4m3) LAUNCH_GATHER8(64, true); else LAUNCH_GATHER8(64, false); }
+#undef LAUNCH_GATHER8
+    } else if (e4m3)
       gather_kernel<true><<<grid, 256, 0, stream>>>(K, V, kv_layer_stride, kv_head_stride, (__half*)retrK, (__half*)retrV,
                                                     r_layer_stride, r_head_stride, idx, H, sel, chunk * d, d, Ke, Ve);
     else

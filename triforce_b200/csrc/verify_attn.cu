@@ -20,7 +20,8 @@
 //     "Head" below means KV head; MHA is grp = 1 and runs the same code.
 //   * an E4M3 store (tf_verify_attn_e4m3, the format of common.cuh): the same kernel with KV = __nv_fp8_e4m3.  A stage carries
 //     the 64-key code tiles (TMA) and the tiles' 64 + 64 exponents (bulk copy); twice the stages keep the fp16 ring's bytes in
-//     flight.  No calibrated split, L2 prefetch or tree mode.
+//     flight.  No calibrated split, L2 prefetch or tree mode.  Over an E4M3 retrieval cache (tf_verify_attn_e4m3_clean) the
+//     producer fills the ring with code tiles and exponents of the clean region before pdl_wait, as the fp16 kernel does.
 //   * the split is equal by default.  SMs need not all pull the same HBM bandwidth (GPC-level sharing; per-CTA
 //     %globaltimer stamps show it, tools/attn_timing.py), so under an equal split the kernel waits on the slowest GPCs.
 //     tf_verify_attn_calibrate
@@ -938,9 +939,10 @@ int tf_verify_attn_gqa(const void* q, const void* k_tensormap, const void* v_ten
                           workspace, workspace_bytes, variant, nullptr, 0, false, clean_keys, stream);
 }
 
-int tf_verify_attn_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
-                        long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv,
-                        int d, float scale, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+static int verify_attn_e4m3_impl(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp,
+                                 const int8_t* v_exp, long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max,
+                                 int R, int Hq, int Hkv, int d, float scale, void* out, void* workspace, size_t workspace_bytes,
+                                 int clean_keys, tf_stream_t stream) {
   const int grp = gqa_group(Hq, Hkv, "tf_verify_attn_e4m3");
   if (grp == 0) return TF_ERR_INVALID;
   TF_CHECK_ARG(k_exp && v_exp, "tf_verify_attn_e4m3: NULL exponent pointer");
@@ -950,7 +952,23 @@ int tf_verify_attn_e4m3(const void* q, const void* k_tensormap, const void* v_te
   TF_CHECK_ARG(kv_len_max <= cap && (kv_len_dev || kv_len_host <= cap), "tf_verify_attn_e4m3: kv_len (%d, max %d) exceeds cap %lld",
                kv_len_host, kv_len_max, cap);
   return verify_attn_impl(q, k_tensormap, v_tensormap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hkv, grp, d, scale, out,
-                          workspace, workspace_bytes, 0, nullptr, 0, false, 0, stream, nullptr, 0, k_exp, v_exp, cap);
+                          workspace, workspace_bytes, 0, nullptr, 0, false, clean_keys, stream, nullptr, 0, k_exp, v_exp, cap);
+}
+
+int tf_verify_attn_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                        long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max, int R, int Hq, int Hkv,
+                        int d, float scale, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  return verify_attn_e4m3_impl(q, k_tensormap, v_tensormap, k_exp, v_exp, cap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hq, Hkv, d,
+                               scale, out, workspace, workspace_bytes, 0, stream);
+}
+
+int tf_verify_attn_e4m3_clean(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                              long long cap, int layer, int kv_len_host, const int32_t* kv_len_dev, int kv_len_max, int R, int Hq,
+                              int Hkv, int d, float scale, void* out, void* workspace, size_t workspace_bytes, int clean_keys,
+                              tf_stream_t stream) {
+  TF_CHECK_ARG(clean_keys >= 0 && clean_keys <= cap, "tf_verify_attn_e4m3_clean: clean_keys (%d) outside [0, cap %lld]", clean_keys, cap);
+  return verify_attn_e4m3_impl(q, k_tensormap, v_tensormap, k_exp, v_exp, cap, layer, kv_len_host, kv_len_dev, kv_len_max, R, Hq, Hkv, d,
+                               scale, out, workspace, workspace_bytes, clean_keys, stream);
 }
 
 int tf_verify_attn_prefetch(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len_host,

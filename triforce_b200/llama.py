@@ -177,6 +177,7 @@ class LlamaModel:
         # retrieval-verify attention prefetching the o_proj weights into L2 while it is latency-bound (tf_verify_attn_prefetch).
         # OPT-IN (not measured faster on H100): the requests
         # compete with the K/V tiles of the attention they ride on, and o_proj's own ring fill under PDL already covers its start.
+        # It has no e4m3 path: over an E4M3 retrieval cache the verify attention never prefetches.
         self.attn_prefetch = os.environ.get("TRIFORCE_ATTN_PREFETCH", "0") == "1" and self.use_stream_linear
         self._tc_ws, self._tc_ws_key = None, None
 
@@ -500,6 +501,12 @@ class LlamaModel:
                 ops.verify_attn_e4m3(q_out, st, l, n if use_device_len else old_len + n, n, Hl, Hkv, d, self.scale, out, ws,
                                      kv_len_dev=kv_cache.seq_len_dev if use_device_len else None)
                 return out
+            if spec and kv_dtype_of(graph_cache) == "e4m3":  # E4M3 retrieval cache: quantized append, PDL verify with the early ring fill
+                st, Hkv = graph_cache.e4m3, self.local_num_kv_heads
+                ops.rope_append_e4m3(qkv, Hl, Hkv, d, self.cos, self.sin, q_out, st, l, pos_ids=pos32, slot0=graph_cache.max_budget)
+                ops.verify_attn_e4m3(q_out, st, l, graph_cache.real_budget, n, Hl, Hkv, d, self.scale, out, ws,
+                                     clean_keys=graph_cache.max_budget)  # rope_append wrote slots >= budget only
+                return out
             if spec:
                 self._rope_append(qkv, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
                                   slot0=graph_cache.max_budget)
@@ -531,15 +538,7 @@ class LlamaModel:
             if not first:  # cache.py:191-194 per-layer tail copy (empty in the on-chip flow: seq_len <= prefill)
                 L = len(self.layers)
                 for l in range(L):
-                    seq = old_len + (1 if l == L - 1 else 0)
-                    m = seq - graph_cache.prefill
-                    if m > 0 and e4m3:
-                        ops.tail_update_e4m3(kv_cache.e4m3, graph_cache.key_store, graph_cache.value_store, graph_cache.prefill,
-                                             graph_cache.max_budget, seq, layer0=l, n_layers=1)
-                    elif m > 0:
-                        B, P = graph_cache.max_budget, graph_cache.prefill
-                        graph_cache.key_store[l, :, B - m:B] = kv_cache.key_store[l, :, P:seq]
-                        graph_cache.value_store[l, :, B - m:B] = kv_cache.value_store[l, :, P:seq]
+                    graph_cache.copy_tail_layer(kv_cache, old_len + (1 if l == L - 1 else 0), l)
         return logits.unsqueeze(0)
 
     # --- tree (Sequoia) ------------------------------------------------------------------------------------------------

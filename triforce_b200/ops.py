@@ -115,9 +115,10 @@ def rope_append_e4m3(qkv: torch.Tensor, Hq: int, Hkv: int, d: int, cos, sin, q_o
 
 
 def verify_attn_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float, out,
-                     workspace, kv_len_dev=None, kv_len_max: Optional[int] = None):
-    """verify_attn_gqa (causal, Hq == Hkv is MHA) over the e4m3 store (tf_verify_attn_e4m3); workspace from
-    verify_attn_gqa_workspace.  Rows are cut into bottom-right aligned blocks of gqa_row_block(Hq, Hkv) token rows."""
+                     workspace, kv_len_dev=None, kv_len_max: Optional[int] = None, clean_keys: int = 0):
+    """verify_attn_gqa (causal, Hq == Hkv is MHA) over the e4m3 store (tf_verify_attn_e4m3_clean); workspace from
+    verify_attn_gqa_workspace.  Rows are cut into bottom-right aligned blocks of gqa_row_block(Hq, Hkv) token rows.
+    `clean_keys`: keys the preceding kernel does not write (see verify_attn), loaded before the launch waits on it."""
     require_cuda(q, out, workspace)
     _f16c(q, "q")
     assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and out.shape == q.shape
@@ -130,10 +131,11 @@ def verify_attn_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: i
         raise ValueError(f"{Hq // Hkv} query heads per KV head exceed the {VERIFY_MAX_ROWS} rows of a verify-attention CTA")
     for r0 in range(0, R, step):
         r1 = min(R, r0 + step)
-        check(lib().tf_verify_attn_e4m3(q[r0:r1].data_ptr(), store.k_ptr, store.v_ptr, store.k_exp.data_ptr(), store.v_exp.data_ptr(),
-                                        cap, layer, kv_len - (R - r1), ptr(kv_len_dev), min(kv_len_max, cap), r1 - r0, Hq, Hkv, d,
-                                        scale, out[r0:r1].data_ptr(), workspace.data_ptr(), workspace.numel(), stream_ptr()),
-              "tf_verify_attn_e4m3")
+        check(lib().tf_verify_attn_e4m3_clean(q[r0:r1].data_ptr(), store.k_ptr, store.v_ptr, store.k_exp.data_ptr(),
+                                              store.v_exp.data_ptr(), cap, layer, kv_len - (R - r1), ptr(kv_len_dev),
+                                              min(kv_len_max, cap), r1 - r0, Hq, Hkv, d, scale, out[r0:r1].data_ptr(),
+                                              workspace.data_ptr(), workspace.numel(), clean_keys, stream_ptr()),
+              "tf_verify_attn_e4m3_clean")
         COUNTER.n += 1
 
 
@@ -172,6 +174,64 @@ def tail_update_e4m3(store: E4m3Store, retr_key_store, retr_value_store, prefill
                                     store.v_exp[layer0].data_ptr(), kc.stride(0), kc.stride(1), retr_key_store[layer0].data_ptr(),
                                     retr_value_store[layer0].data_ptr(), retr_key_store.stride(0), retr_key_store.stride(1), n, H, d,
                                     prefill, budget, seq_len, ptr(seq_len_dev), max_new, stream_ptr()), "tf_tail_update_e4m3")
+    COUNTER.n += 1
+
+
+def _full_store(src):
+    """(K, V, K exponents, V exponents, layer stride, head stride, Hkv, d) of a full-KV store: an E4m3Store, or the fp16
+    (key_store, value_store) pair (NULL exponents)."""
+    if isinstance(src, E4m3Store):
+        L, H, cap, d = src.shape
+        return src.k_codes, src.v_codes, src.k_exp, src.v_exp, src.k_codes.stride(0), src.k_codes.stride(1), H, d
+    k, v = src
+    require_cuda(k, v)
+    _f16c(k, "key_store")
+    assert k.is_contiguous() and v.is_contiguous() and v.shape == k.shape
+    return k, v, None, None, k.stride(0), k.stride(1), k.shape[1], k.shape[3]
+
+
+def retrieval_build_to_e4m3(src, q, cache: E4m3Store, prefill: int, chunk: int, budget: int, layer0: int = 0,
+                            n_layers: Optional[int] = None, out_idx=None, out_scores=None):
+    """The retrieval build into an E4M3 retrieval cache (tf_retrieval_build_to_e4m3): `src` is the full store, an E4m3Store or the
+    fp16 (key_store, value_store) pair; q [n_layers,Hq,d] (Hq > Hkv: the "group_sum" rule).  Scoring and top-k are those of
+    retrieval_build / retrieval_build_gqa / retrieval_build_e4m3; the cache receives the quantized rows, or the store's own codes."""
+    K, V, Ke, Ve, ls, hs, Hkv, d = _full_store(src)
+    require_cuda(q)
+    _f16c(q, "q")
+    n = q.shape[0] if n_layers is None else n_layers
+    Hq = q.shape[1]
+    assert q.is_contiguous() and q.shape == (n, Hq, d), (q.shape, (n, Hq, d))
+    assert cache.shape[1] == Hkv and cache.shape[3] == d and cache.shape[2] >= budget, (cache.shape, Hkv, d, budget)
+    ws_bytes = lib().tf_retrieval_build_workspace_bytes(n, Hkv, d, prefill, chunk, budget)
+    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=q.device)
+    if out_idx is not None:
+        assert out_idx.dtype == torch.int32 and out_idx.is_contiguous() and out_idx.shape == (n, Hkv, budget // chunk)
+    if out_scores is not None:
+        assert out_scores.dtype == torch.float16 and out_scores.is_contiguous() and out_scores.shape == (n, Hkv, prefill // chunk)
+    rc = cache.k_codes
+    check(lib().tf_retrieval_build_to_e4m3(K[layer0].data_ptr(), V[layer0].data_ptr(), ptr(None if Ke is None else Ke[layer0]),
+                                           ptr(None if Ve is None else Ve[layer0]), ls, hs, q.data_ptr(), n, Hq, Hkv, d, prefill, chunk,
+                                           budget, rc[layer0].data_ptr(), cache.v_codes[layer0].data_ptr(),
+                                           cache.k_exp[layer0].data_ptr(), cache.v_exp[layer0].data_ptr(), rc.stride(0), rc.stride(1),
+                                           ptr(out_idx), ptr(out_scores), ws.data_ptr(), ws.numel(), stream_ptr()),
+          "tf_retrieval_build_to_e4m3")
+    COUNTER.n += 3
+
+
+def tail_update_to_e4m3(src, cache: E4m3Store, prefill: int, budget: int, seq_len: int, seq_len_dev=None, max_new: int = 0,
+                        layer0: int = 0, n_layers: Optional[int] = None):
+    """tail_update into an E4M3 retrieval cache (tf_tail_update_to_e4m3), layers [layer0, layer0+n): `src` an E4m3Store (codes and
+    exponents copied) or the fp16 (key_store, value_store) pair (rows quantized)."""
+    K, V, Ke, Ve, ls, hs, H, d = _full_store(src)
+    L = K.shape[0]
+    assert cache.shape[1] == H and cache.shape[3] == d and cache.shape[2] >= budget, (cache.shape, H, d, budget)
+    n = L - layer0 if n_layers is None else n_layers
+    rc = cache.k_codes
+    check(lib().tf_tail_update_to_e4m3(K[layer0].data_ptr(), V[layer0].data_ptr(), ptr(None if Ke is None else Ke[layer0]),
+                                       ptr(None if Ve is None else Ve[layer0]), ls, hs, rc[layer0].data_ptr(),
+                                       cache.v_codes[layer0].data_ptr(), cache.k_exp[layer0].data_ptr(), cache.v_exp[layer0].data_ptr(),
+                                       rc.stride(0), rc.stride(1), n, H, d, prefill, budget, seq_len, ptr(seq_len_dev), max_new,
+                                       stream_ptr()), "tf_tail_update_to_e4m3")
     COUNTER.n += 1
 
 

@@ -17,7 +17,7 @@ from typing import Dict, Optional
 import torch
 import torch.distributed as dist
 
-from .cache import FlashSimpleCache, RetrievalCache, RetrievalCacheSeqouia, StreamingLLMEvictionCache
+from .cache import KV_DTYPES, FlashSimpleCache, RetrievalCache, RetrievalCacheSeqouia, StreamingLLMEvictionCache
 from .config import LlamaShape, named_config
 from .engine import GraphInferenceEngine
 from .llama import LlamaModel
@@ -228,7 +228,8 @@ class DistributedLlama:
     def __init__(self, model_name_or_path: str, dtype=torch.float16, kv_offload=False, on_chip_layers=32, local_rank=0, world_size=1,
                  prefill=32768, bsz=1, gen_len=256, retrieval_budget=4096, retrieval_chunk_size=8, gamma=6, temperature=0.6,
                  top_p=0.9, ssl=0, draft=None, draft_cache=None, flash_attn=True, config: Optional[LlamaShape] = None,
-                 tree_size: int = 0, kv_dtype: str = "fp16", weight_dtype: str = "fp16") -> None:
+                 tree_size: int = 0, kv_dtype: str = "fp16", weight_dtype: str = "fp16", retrieval_dtype: str = "fp16") -> None:
+        """`retrieval_dtype`: the rank-local retrieval cache in fp16 or E4M3 (RetrievalCache kv_dtype); the seams never see it."""
         assert bsz == 1
         if kv_dtype != "fp16":
             raise NotImplementedError(f"DistributedLlama (tensor parallel) keeps an fp16 full-KV store; kv_dtype={kv_dtype!r} is not supported")
@@ -244,6 +245,9 @@ class DistributedLlama:
         self.retrieval_budget, self.retrieval_chunk_size = retrieval_budget, retrieval_chunk_size
         self.temperature, self.top_p, self.gamma = temperature, top_p, gamma
         self.draft, self.draft_cache = draft, draft_cache
+        if retrieval_dtype not in KV_DTYPES:
+            raise ValueError(f"retrieval_dtype must be one of {KV_DTYPES}, got {retrieval_dtype!r}")
+        self.retrieval_dtype = retrieval_dtype
         self.tree_size = tree_size  # > 0: Sequoia mode (models/TP_llama_tree.py), retrieval cache reserves tree slots
         self.hidden_size = self.config.hidden_size
         self.num_heads = self.config.num_attention_heads
@@ -263,10 +267,12 @@ class DistributedLlama:
         budget = self.retrieval_budget if self.retrieval_budget > 0 else self.retrieval_chunk_size
         if self.tree_size > 0:
             self.retrieval_cache = RetrievalCacheSeqouia(self.model, max_budget=budget, prefill=self.prefill_len,
-                                                         chunk_size=self.retrieval_chunk_size, tree_size=self.tree_size)
+                                                         chunk_size=self.retrieval_chunk_size, tree_size=self.tree_size,
+                                                         kv_dtype=self.retrieval_dtype)
         else:
             self.retrieval_cache = RetrievalCache(self.model, max_budget=budget, prefill=self.prefill_len,
-                                                  chunk_size=self.retrieval_chunk_size, gamma=self.gamma)
+                                                  chunk_size=self.retrieval_chunk_size, gamma=self.gamma,
+                                                  kv_dtype=self.retrieval_dtype)
         if self.draft is not None:
             self.graph_engine = GraphInferenceEngine(self.model, self.kv_cache, self.retrieval_cache, self.draft, self.draft_cache)
             self.graph_engine.engine.draft_prefill_chunk = 128  # TP_llama.py:118-126
