@@ -477,6 +477,9 @@ int tf_allreduce_oneshot(void* const* peer_buffers, void* multicast_buffer, int 
  * tf_norm_logits: utils/sampling.py:43-60 (norm_logits) incl. the top-p filter :16-27 — logits/T, descending stable
  *   sort, softmax, cumulative sum, keep the prefix whose exclusive cumulative mass <= top_p (first token always kept),
  *   renormalise.  fp32 in/out, one CTA per row, rows x V with V <= TF_SAMPLING_MAX_VOCAB.  top_p >= 1 keeps everything.
+ *   temperature == 0 is greedy decoding, the T -> 0 limit: each row is one-hot (1.0 / 0.0) at its first maximal logit, the
+ *   index torch.argmax returns (ties to the lowest index, NaN counts as maximal); top_p has no effect and no exp is taken.
+ *   A negative (or NaN) temperature is TF_ERR_INVALID.
  * tf_sample_argmax: utils/sampling.py:63-65 — torch.multinomial(p, 1) on CUDA is argmax(p / Exp(1)-noise); the noise
  *   is an input so the caller decides the random stream.  Writes an int64 token per row (first index on ties).
  * tf_residual_probs: utils/sampling.py:68-75 (max_fn): out = relu(p-q) / sum(relu(p-q)).
@@ -512,6 +515,9 @@ int tf_residual_probs(const float* p, const float* q, int V, float* out, tf_stre
  *   (succ_off int32 [T+1], succ int32), uniforms consumed one per examined child.  out int32[32]: [0] accepted nodes,
  *   [1] -1 (all children rejected) / -2 (leaf), [2] uniforms consumed, [3] terminal (token 0 or 2 accepted), [4] residual
  *   is NaN, [8..8+max_accept) accepted node ids.  `residual` [V] = the distribution the next token is drawn from.
+ *   temperature == 0 is the greedy walk: at each node it follows the child whose token is torch.argmax of the node's target
+ *   row and stops when no child carries it; `residual` is one-hot at that argmax, no uniform is consumed (out[2] = 0) and
+ *   draft_logits is neither read nor written.  temperature < 0 is TF_ERR_INVALID.
  */
 int tf_tree_accept_walk(const float* target_probs, float* draft_logits, const int64_t* verify_tokens, const int32_t* succ_off,
                         const int32_t* succ, const float* uniforms, float temperature, int V, int max_accept, int32_t* out,

@@ -17,6 +17,14 @@ from typing import List, Optional
 import numpy as np
 import torch
 
+def _temperature(text: str) -> float:
+    """`--temp`: a temperature >= 0.  0 is greedy decoding (every probability row one-hot at the argmax of its logits)."""
+    t = float(text)
+    if not t >= 0.0:  # also refuses NaN
+        raise argparse.ArgumentTypeError(f"temperature must be >= 0, got {text}")
+    return t
+
+
 # (flag, kwargs) in the order of the reference's argparse blocks: on_chip.py:21-40, offloading_TP.py:26-44,
 # offloading_seqouia.py:41-58.  Defaults are the reference's.
 _COMMON_TP_FLAGS = [
@@ -24,7 +32,7 @@ _COMMON_TP_FLAGS = [
     ("--verbose", dict(action="store_true", help="verbose")),
     ("--prefill", dict(type=int, default=130048, help="prefill length")),
     ("--gen_len", dict(type=int, default=256, help="generation length")),
-    ("--temp", dict(type=float, default=0.6, help="temperature")),
+    ("--temp", dict(type=_temperature, default=0.6, help="temperature (0 = greedy decoding)")),
     ("--top_p", dict(type=float, default=0.9, help="top p")),
     ("--dataset", dict(type=str, default="demo", help="dataset")),
     ("--on_chip", dict(type=int, default=0, help="on chip layers (ignored: everything is on chip)")),
@@ -46,7 +54,7 @@ FLAGS = {
         ("--gen_len", dict(type=int, default=256, help="generation length")),
         ("--gamma", dict(type=int, default=6, help="gamma")),
         ("--dataset", dict(type=str, default="gs", help="dataset")),
-        ("--temp", dict(type=float, default=0.6, help="temperature")),
+        ("--temp", dict(type=_temperature, default=0.6, help="temperature (0 = greedy decoding)")),
         ("--top_p", dict(type=float, default=0.9, help="top p")),
         ("--budget", dict(type=int, default=4096)),
         ("--draft_cache_budget", dict(type=int, default=256, help="draft cache budget")),

@@ -108,6 +108,24 @@ __device__ __forceinline__ ArgBest block_argmax(ArgBest b, float* redv, int* red
   return r;
 }
 
+// torch.argmax of row[0, V); every thread returns the winner.  Eight independent loads in flight per thread.
+__device__ __forceinline__ int block_row_argmax(const float* __restrict__ row, int V, float* redv, int* redi) {
+  ArgBest b{-INFINITY, 0x7fffffff};
+  const int step = blockDim.x;
+  int i = threadIdx.x;
+  for (; i + 7 * step < V; i += 8 * step) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v[u] = row[i + u * step];
+#pragma unroll
+    for (int u = 0; u < 8; ++u)
+      if (arg_better(v[u], i + u * step, b.v, b.i)) { b.v = v[u]; b.i = i + u * step; }
+  }
+  for (; i < V; i += step)
+    if (arg_better(row[i], i, b.v, b.i)) { b.v = row[i]; b.i = i; }
+  return block_argmax(b, redv, redi).i;
+}
+
 // IEEE division out of line: the correctly rounded quotient the reference's `/` gives (ATen), without replicating the
 // special-case path of div.rn at every unrolled call site, which would bloat the 25 K-instruction norm_logits body and stall
 // it on instruction fetch.
@@ -316,6 +334,20 @@ __global__ void __launch_bounds__(kNlThreads) norm_logits_kernel(const float* __
   }
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// norm_logits at temperature 0: the T -> 0 limit of the softmax, one-hot at the row's first maximal logit (torch.argmax:
+// ties to the lowest index, NaN counts as maximal).  top_p has no effect: the argmax is always inside the nucleus.  One
+// argmax pass and one store pass per row, no exp, no threshold search.
+// --------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads) one_hot_argmax_kernel(const float* __restrict__ logits, long long row_stride, int V,
+                                                                  float* __restrict__ probs) {
+  __shared__ float redv[32];
+  __shared__ int redi[32];
+  const int win = block_row_argmax(logits + (size_t)blockIdx.x * row_stride, V, redv, redi);
+  float* out = probs + (size_t)blockIdx.x * V;
+  for (int i = threadIdx.x; i < V; i += kThreads) out[i] = i == win ? 1.f : 0.f;
+}
+
 __global__ void __launch_bounds__(kThreads) sample_argmax_kernel(const float* __restrict__ probs, long long ps,
                                                                  const float* __restrict__ expo, long long es, int V,
                                                                  int64_t* __restrict__ out) {
@@ -463,21 +495,43 @@ __global__ void __launch_bounds__(kThreads) verify_resample_kernel(const float* 
 //   otherwise p = relu(p - q) / sum and draft_logits[cur][token] = -FLT_MAX (so the next q excludes it).  An accepted child
 //   becomes `cur` (tokens 0 / 2 end the generation: "terminal"); when every child is rejected, or a leaf is reached, the
 //   current p is the distribution the next token is drawn from.
+// Greedy walk (temperature 0, `greedy` != 0): at node `cur` the walk follows the child whose token is torch.argmax of
+//   target_probs[cur] and stops when no child carries it; `residual` is then one-hot at that argmax, so the next token is
+//   the target's greedy token at the last accepted node.  No uniform is consumed and draft_logits is neither read nor
+//   written.  This is the T -> 0 limit of the walk above: with one-hot target rows, the accept ratio is 1 for the argmax
+//   child and 0 for every other one.
 // out (int32[32]): [0] accepted count, [1] code (-1 all children rejected, -2 leaf), [2] uniforms consumed, [3] terminal,
 //                  [4] residual has NaN / zero mass, [8..] accepted node ids.
 // --------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) tree_accept_walk_kernel(const float* __restrict__ target_probs, float* __restrict__ draft_logits,
                                                                     const int64_t* __restrict__ verify_tokens,
                                                                     const int32_t* __restrict__ succ_off, const int32_t* __restrict__ succ,
-                                                                    const float* __restrict__ uniforms, float inv_T, int V,
+                                                                    const float* __restrict__ uniforms, float inv_T, int greedy, int V,
                                                                     int max_accept, int32_t* __restrict__ out,
                                                                     float* __restrict__ residual, float* __restrict__ pbuf) {
   __shared__ float redf[32];
+  __shared__ int redi[32];
   __shared__ int s_accept;
   const int tid = threadIdx.x;
   int cur = 0, n_acc = 0, used = 0, code = 0, terminal = 0;
   bool nan_res = false;
-  while (true) {
+  while (greedy) {
+    const int c0 = succ_off[cur], c1 = succ_off[cur + 1];
+    const int best = block_row_argmax(target_probs + (size_t)cur * V, V, redf, redi);
+    int child = -1;
+    for (int c = c0; c < c1 && child < 0; ++c)
+      if (verify_tokens[succ[c]] == best) child = succ[c];
+    if (child < 0) {
+      for (int i = tid; i < V; i += kThreads) residual[i] = i == best ? 1.f : 0.f;
+      code = c0 == c1 ? -2 : -1;
+      break;
+    }
+    if (tid == 0 && n_acc < max_accept) out[8 + n_acc] = child;
+    ++n_acc;
+    cur = child;
+    if (best == 0 || best == 2) { terminal = 1; break; }
+  }
+  while (!greedy) {  // the sampled walk (T > 0)
     const int c0 = succ_off[cur], c1 = succ_off[cur + 1];
     const float* p = target_probs + (size_t)cur * V;  // accept_step starts from the node's own target row
     if (c0 == c1) {  // leaf
@@ -561,8 +615,13 @@ int tf_norm_logits(const float* logits, long long row_stride, int rows, int V, f
   (void)workspace; (void)workspace_bytes;
   TF_CHECK_ARG(logits && probs && rows >= 0 && V > 0, "tf_norm_logits: bad arguments");
   TF_CHECK_SUPPORTED(V <= TF_SAMPLING_MAX_VOCAB, "tf_norm_logits: vocab %d > %d", V, TF_SAMPLING_MAX_VOCAB);
-  TF_CHECK_ARG(temperature > 0.f, "tf_norm_logits: temperature must be > 0");
+  TF_CHECK_ARG(temperature >= 0.f, "tf_norm_logits: temperature must be >= 0");
   if (rows == 0) return TF_OK;
+  if (temperature == 0.f) {
+    one_hot_argmax_kernel<<<rows, kThreads, 0, (cudaStream_t)stream_>>>(logits, row_stride, V, probs);
+    TF_CHECK_LAUNCH();
+    return TF_OK;
+  }
   const size_t smem = (size_t)TF_SAMPLING_MAX_VOCAB * sizeof(uint32_t);
   TF_ENSURE_DYNAMIC_SMEM(norm_logits_kernel, smem);
   norm_logits_kernel<<<rows, kNlThreads, smem, (cudaStream_t)stream_>>>(logits, row_stride, V, temperature, top_p, probs);
@@ -607,9 +666,11 @@ int tf_tree_accept_walk(const float* target_probs, float* draft_logits, const in
   using namespace tf;
   TF_CHECK_ARG(target_probs && draft_logits && verify_tokens && succ_off && succ && uniforms && out && residual && scratch_V,
                "tf_tree_accept_walk: NULL pointer");
-  TF_CHECK_ARG(V > 0 && temperature > 0.f && max_accept >= 1 && max_accept <= 24, "tf_tree_accept_walk: bad V / temperature / max_accept");
+  TF_CHECK_ARG(V > 0 && temperature >= 0.f && max_accept >= 1 && max_accept <= 24, "tf_tree_accept_walk: bad V / temperature / max_accept");
+  const int greedy = temperature == 0.f;
   tree_accept_walk_kernel<<<1, kThreads, 0, (cudaStream_t)stream_>>>(target_probs, draft_logits, verify_tokens, succ_off, succ, uniforms,
-                                                                     1.0f / temperature, V, max_accept, out, residual, scratch_V);
+                                                                     greedy ? 0.f : 1.0f / temperature, greedy, V, max_accept, out,
+                                                                     residual, scratch_V);
   TF_CHECK_LAUNCH();
   return TF_OK;
 }

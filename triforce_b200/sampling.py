@@ -32,13 +32,16 @@ def top_k_top_p_filter(logits: torch.Tensor, top_k: int = 0, top_p: float = 0.0)
 
 def norm_logits(logits: torch.Tensor, temperature=0.6, top_k=-1, top_p=0.9) -> torch.Tensor:
     """logits [rows, vocab] fp32 → probabilities after temperature and nucleus filtering (one kernel, one CTA per row).
-    top_k > 0 (never used by the reference's loops) masks with ATen first, then takes the same kernel."""
+    top_k > 0 (never used by the reference's loops) masks with ATen first, then takes the same kernel.
+    temperature 0 is greedy decoding: each row is one-hot at torch.argmax of its logits (top_k and top_p change nothing)."""
     assert logits.dim() == 2
     if logits.dtype != torch.float32:
         logits = logits.float()
     if logits.stride(-1) != 1:
         logits = logits.contiguous()
     if top_k is not None and top_k > 0:
+        if temperature == 0:
+            return ops.norm_logits(_top_k_mask_(logits.clone(), top_k), 0.0, float(top_p))
         return ops.norm_logits(_top_k_mask_(logits / temperature, top_k), 1.0, float(top_p))
     return ops.norm_logits(logits, float(temperature), float(top_p))
 

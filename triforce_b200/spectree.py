@@ -76,7 +76,15 @@ def get_residual(p: torch.Tensor, q: torch.Tensor) -> torch.Tensor:
 def create_sampling_callable(num_samples: int, temperature: float = 0.6):
     """Sampling WITHOUT replacement of `num_samples` children per parent row: the Gumbel/exponential-race trick of
     test/offloading_seqouia.py:29-39 — `(rand.log() / softmax(logits / T)).topk(k)` (rank-0 + broadcast in the reference;
-    here every rank evaluates it on identical inputs)."""
+    here every rank evaluates it on identical inputs).
+
+    temperature 0 (greedy): the T -> 0 limit of the race, the `num_samples` largest logits of each row, ties to the lower
+    index (a stable descending sort; NaN sorts first, as torch.argmax counts it maximal).  The noise is not read."""
+    if temperature == 0:
+        def greedy_children(sampling_logits: torch.Tensor, static_rand: torch.Tensor) -> torch.Tensor:
+            return torch.sort(sampling_logits, dim=-1, descending=True, stable=True).indices[:, :num_samples].flatten()
+        return greedy_children
+
     def sampling_without_replacement(sampling_logits: torch.Tensor, static_rand: torch.Tensor) -> torch.Tensor:
         sampling_q = torch.softmax(sampling_logits / temperature, dim=-1)
         return (static_rand.log() / sampling_q).topk(k=num_samples).indices.flatten()
