@@ -250,6 +250,15 @@ int tf_tree_attn_tc(const void* q, const void* k_tensormap, const void* v_tensor
 int tf_tree_attn_tc_gqa(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int Hq,
                         int Hkv, int d, float scale, const uint32_t* tree_mask, int tree_cols, int causal, void* out,
                         void* workspace, size_t workspace_bytes, tf_stream_t stream);
+/* tf_tree_attn_tc_e4m3: tf_tree_attn_tc_gqa (Hq == Hkv is MHA) over an E4M3 store — tensor maps from
+ *   tf_kv_tensormap_encode_e4m3 with box_keys = TF_VERIFY_BOX_KEYS, exponents [L][Hkv][cap] 16-byte aligned, cap % TF_VERIFY_BOX_KEYS
+ *   == 0, kv_len <= cap.  A converter warpgroup expands each 128-key code tile into the fp16 shared-memory tile tf_tree_attn_tc
+ *   would load from a store holding D = fp16_rn(code * 2^e), and the consumers run unchanged: the output is bit-identical to
+ *   tf_tree_attn_tc_gqa over the dequantized store.  Workspace from tf_tree_attn_tc_workspace_bytes(R, Hq, kv_len_max).  No causal
+ *   mode (prompts attend over an fp16 scratch) and no score hook. */
+int tf_tree_attn_tc_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                         long long cap, int layer, int kv_len, int R, int Hq, int Hkv, int d, float scale, const uint32_t* tree_mask,
+                         int tree_cols, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream);
 
 /* Init-time load balancing of tf_verify_attn (no reference counterpart; the reference has no such knob).  The kernel cuts
  * its (head, key-tile) axis into one contiguous range per CTA.  Where the SMs of a GPU do not all pull the same HBM bandwidth,
@@ -298,6 +307,10 @@ int tf_window_slide(void* K, void* V, long long layer_stride, long long head_str
  *   accepted nodes (src_idx_dev[i], absolute slots) are packed to slots dst_start + i of every (layer, head), clone semantics. */
 int tf_kv_compact(void* K, void* V, long long layer_stride, long long head_stride, int n_layers, int H, int d,
                   const int32_t* src_idx_dev, int n, int dst_start, tf_stream_t stream);
+/* tf_kv_compact_e4m3: tf_kv_compact over a contiguous E4M3 store (codes [L][H][cap][d] uint8, exponents [L][H][cap] int8, K
+ *   and V): codes and exponents of rows src_idx_dev[i] go to row dst_start + i, bit for bit, clone semantics, one launch. */
+int tf_kv_compact_e4m3(void* k_codes, void* v_codes, int8_t* k_exp, int8_t* v_exp, long long cap, int n_layers, int H, int d,
+                       const int32_t* src_idx_dev, int n, int dst_start, tf_stream_t stream);
 
 /* ---- elementwise glue of the decoder layer (fp16 rounding points of the reference) -----------------------------
  * tf_add_rmsnorm: h = fp16(h + delta) (delta may be NULL); out = fp16(w * fp16(h * rsqrt(mean(h^2) + eps)))

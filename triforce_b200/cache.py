@@ -124,6 +124,14 @@ class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
         require_fp16_store(self, "gather_kv_incremental")
         super().gather_kv_incremental(indices, offset)
 
+    def gather_kv_incremental_e4m3(self, indices, offset: int):
+        """gather_kv_incremental over an E4M3 store (tf_kv_compact_e4m3): the accepted nodes' codes and exponents, bit for bit."""
+        if kv_dtype_of(self) != "e4m3":
+            raise NotImplementedError(f"gather_kv_incremental_e4m3 needs an E4M3 full-KV store; this one is {kv_dtype_of(self)}")
+        idx = torch.tensor([int(i) + offset for i in indices], dtype=torch.int32, device=self.key_store.device)
+        ops.kv_compact_e4m3(self.e4m3, idx, offset)
+        self.seq_len = offset + len(indices)
+
     def sync_seq_len_to_device(self):
         """Mirror the Python `seq_len` into `seq_len_dev` on the current stream (graphs read kv_len from there).
         Stream-ordered (`fill_` carries the value as a kernel argument), so the host may run ahead of the GPU."""

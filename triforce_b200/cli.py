@@ -41,10 +41,17 @@ _COMMON_TP_FLAGS = [
     ("--file", dict(type=str, default="")),
     ("--seed", dict(type=int, default=1, help="seed")),
 ]
-# addition (not in the reference) of on_chip and offloading_TP; the Sequoia tree path keeps an fp16 retrieval cache
+# additions (not in the reference) of on_chip, offloading_TP and offloading_seqouia; the Sequoia tree path keeps an fp16 retrieval
+# cache, and the full-KV store and the weights take E4M3 on one GPU only
 _RETRIEVAL_DTYPE_FLAG = ("--retrieval_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
                                                    help="retrieval cache: fp16, or FP8 E4M3 with a per-row power-of-two scale "
                                                         "(changes acceptance, not the target's numerics)"))
+_KV_DTYPE_FLAG = ("--kv_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
+                                     help="full-KV store: fp16, or FP8 E4M3 with a per-row power-of-two scale (changes the target's "
+                                          "numerics)"))
+_WEIGHT_DTYPE_FLAG = ("--weight_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
+                                             help="target projection weights: fp16, or FP8 E4M3 with a per-row power-of-two scale "
+                                                  "(changes the target's numerics)"))
 FLAGS = {
     "on_chip": [
         ("--target", dict(type=str, default="llama-7B-128K", help="target model")),
@@ -63,15 +70,12 @@ FLAGS = {
         ("--target_path", dict(type=str, default=None, help="local HF checkpoint dir of the target")),
         ("--draft_path", dict(type=str, default=None, help="local HF checkpoint dir of the draft")),
         ("--seed", dict(type=int, default=0)),
-        ("--kv_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
-                            help="full-KV store: fp16, or FP8 E4M3 with a per-row power-of-two scale (changes the target's numerics)")),
-        ("--weight_dtype", dict(type=str, default="fp16", choices=["fp16", "e4m3"],
-                                help="target projection weights: fp16, or FP8 E4M3 with a per-row power-of-two scale "
-                                     "(changes the target's numerics)")),
+        _KV_DTYPE_FLAG,
+        _WEIGHT_DTYPE_FLAG,
         _RETRIEVAL_DTYPE_FLAG,
     ],
     "offloading_TP": _COMMON_TP_FLAGS + [("--gamma", dict(type=str, default=6)), _RETRIEVAL_DTYPE_FLAG],
-    "offloading_seqouia": _COMMON_TP_FLAGS + [("--tree_size", dict(type=str, default="512"))],
+    "offloading_seqouia": _COMMON_TP_FLAGS + [("--tree_size", dict(type=str, default="512")), _KV_DTYPE_FLAG, _WEIGHT_DTYPE_FLAG],
 }
 
 # the hub ids the reference maps its `--target` names to (offloading_TP.py:52-61); resolved to shapes by triforce_b200.tp
@@ -262,7 +266,7 @@ def run_offloading_seqouia(argv: Optional[List[str]] = None) -> None:
 
     from .spectree import SpecTree, get_residual, load_grow_map
     from .synth import cuda_state_dict
-    from .tp import DistributedLlama
+    from .tp import DistributedLlama, SingleGpuLlama
 
     args, local_rank, world_size, device, hub = _tp_setup("offloading_seqouia", argv)
     grow_map = load_grow_map(args.tree_size)  # reference: torch.load(f'tree/{args.tree_size}.pt')
@@ -270,10 +274,15 @@ def run_offloading_seqouia(argv: Optional[List[str]] = None) -> None:
     if args.baseline:
         _tp_baseline(args, hub, local_rank, world_size, device, prompts[0][:, :args.prefill].to(device))
         _finish_distributed()
-    llm = DistributedLlama(model_name_or_path=hub, local_rank=local_rank, world_size=world_size, prefill=args.prefill,
-                           gen_len=args.gen_len, temperature=args.temp, top_p=args.top_p, flash_attn=True,
-                           retrieval_budget=args.budget, kv_offload=True, on_chip_layers=args.on_chip, tree_size=grow_map["size"])
-    llm.init_parameters(state_dict=cuda_state_dict(llm.config, seed=1, device=device), cuda_graphs=False)
+    # E4M3 formats run on one GPU (SingleGpuLlama refuses world_size > 1).  Their fp16 weights are drawn on the GPU but kept in
+    # host memory, so they are never resident beside the E4M3 store.
+    host = args.kv_dtype == "e4m3" or args.weight_dtype == "e4m3"
+    engine = SingleGpuLlama if host else DistributedLlama
+    llm = engine(model_name_or_path=hub, local_rank=local_rank, world_size=world_size, prefill=args.prefill,
+                 gen_len=args.gen_len, temperature=args.temp, top_p=args.top_p, flash_attn=True,
+                 retrieval_budget=args.budget, kv_offload=True, on_chip_layers=args.on_chip, tree_size=grow_map["size"],
+                 kv_dtype=args.kv_dtype, weight_dtype=args.weight_dtype)
+    llm.init_parameters(state_dict=cuda_state_dict(llm.config, seed=1, device=device, host=host), cuda_graphs=False)
     tree = SpecTree(engine=llm, temperature=args.temp, top_p=args.top_p, max_length=args.prefill + args.gen_len, grow_map=grow_map,
                     residual_graph=get_residual, tokenizer=SyntheticTokenizer(), vocab_size=llm.config.vocab_size)
     latencies, accepted = [], []

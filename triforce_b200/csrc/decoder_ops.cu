@@ -316,6 +316,33 @@ __global__ void __launch_bounds__(128) kv_compact_kernel(__half* __restrict__ K,
   }
 }
 
+// The same over an E4M3 store ([L][H][cap] rows of d code bytes and one exponent): one CTA per (head, layer) stages the n source
+// rows of K codes, V codes and both exponents in shared memory before it writes any destination row (clone semantics).
+__global__ void __launch_bounds__(128) kv_compact_e4m3_kernel(uint8_t* __restrict__ Kc, uint8_t* __restrict__ Vc, int8_t* __restrict__ Ke,
+                                                              int8_t* __restrict__ Ve, long long cap, int H, int D,
+                                                              const int32_t* __restrict__ src_idx, int n, int dst_start) {
+  extern __shared__ __align__(16) uint8_t csm[];
+  uint4* buf = reinterpret_cast<uint4*>(csm);  // [2][n][D / 16]
+  int8_t* ebuf = reinterpret_cast<int8_t*>(buf + 2 * (size_t)n * (D / 16));  // [2][n]
+  const int h = blockIdx.x, layer = blockIdx.y;
+  const size_t row0 = ((size_t)layer * H + h) * (size_t)cap;
+  const int vec_per_row = D / 16;
+  const int nvec = n * vec_per_row;
+  uint8_t* codes[2] = {Kc + row0 * D, Vc + row0 * D};
+  int8_t* exps[2] = {Ke + row0, Ve + row0};
+  for (int i = threadIdx.x; i < 2 * nvec; i += blockDim.x) {
+    const int w = i / nvec, r = (i % nvec) / vec_per_row, v = i % vec_per_row;
+    buf[i] = *reinterpret_cast<const uint4*>(codes[w] + (size_t)src_idx[r] * D + v * 16);
+  }
+  for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) ebuf[i] = exps[i / n][src_idx[i % n]];
+  __syncthreads();
+  for (int i = threadIdx.x; i < 2 * nvec; i += blockDim.x) {
+    const int w = i / nvec, r = (i % nvec) / vec_per_row, v = i % vec_per_row;
+    *reinterpret_cast<uint4*>(codes[w] + (size_t)(dst_start + r) * D + v * 16) = buf[i];
+  }
+  for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) exps[i / n][dst_start + i % n] = ebuf[i];
+}
+
 // ---- elementwise glue ------------------------------------------------------------------------------------------------
 // One CTA per row, one 16-byte vector (8 halfs) per thread per pass: for hidden = 4096 that is 512 threads with the whole
 // row in registers — a single load, one block reduction, a single store (launch-latency bound: ~3 us).
@@ -608,6 +635,23 @@ int tf_kv_compact(void* K, void* V, long long layer_stride, long long head_strid
   dim3 grid(H, n_layers);
   kv_compact_kernel<<<grid, 128, smem, (cudaStream_t)stream_>>>((__half*)K, (__half*)V, layer_stride, head_stride, d, src_idx_dev, n,
                                                                dst_start);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_kv_compact_e4m3(void* k_codes, void* v_codes, int8_t* k_exp, int8_t* v_exp, long long cap, int n_layers, int H, int d,
+                       const int32_t* src_idx_dev, int n, int dst_start, tf_stream_t stream_) {
+  using namespace tf;
+  TF_CHECK_ARG(k_codes && v_codes && src_idx_dev, "tf_kv_compact_e4m3: NULL pointer");
+  TF_CHECK_ARG(k_exp && v_exp, "tf_kv_compact_e4m3: NULL exponent pointer");
+  TF_CHECK_ARG(n_layers >= 1 && H >= 1 && (d == 64 || d == 128) && cap >= 1, "tf_kv_compact_e4m3: bad arguments");
+  TF_CHECK_ARG((((uintptr_t)k_codes | (uintptr_t)v_codes) & 15) == 0, "tf_kv_compact_e4m3: codes must be 16-byte aligned");
+  TF_CHECK_ARG(n >= 0 && dst_start >= 0 && dst_start + (long long)n <= cap, "tf_kv_compact_e4m3: destination rows outside [0, cap)");
+  if (n == 0) return TF_OK;
+  const size_t smem = (size_t)2 * n * d + 2 * n;
+  TF_CHECK_SUPPORTED(smem <= 48 * 1024, "tf_kv_compact_e4m3: %d rows need %zu B of shared memory", n, smem);
+  kv_compact_e4m3_kernel<<<dim3(H, n_layers), 128, smem, (cudaStream_t)stream_>>>((uint8_t*)k_codes, (uint8_t*)v_codes, k_exp, v_exp, cap,
+                                                                                  H, d, src_idx_dev, n, dst_start);
   TF_CHECK_LAUNCH();
   return TF_OK;
 }

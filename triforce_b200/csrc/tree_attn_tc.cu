@@ -26,6 +26,14 @@
 // coordinate becomes h / grp.  The grp CTAs of a group each stream the same K/V tiles, so KV is read grp times per block
 // instead of once.  That is acceptable here: this kernel is bound by the tensor cores (2·128 FLOP per byte), the group's
 // CTAs run side by side, and the repeated reads hit L2.
+//
+// An E4M3 store (tf_tree_attn_tc_e4m3, the format of common.cuh; MHA or GQA): the wgmma takes both B operands from shared
+// memory as fp16, so the codes become fp16 tiles there and the consumers run unchanged.  Warps 8-11 (the converter warpgroup,
+// 384 threads per CTA) replace the producer warp: thread 0 loads the Q block and the 16 KB code tiles (two 64-key boxes of
+// 128-byte rows, SWIZZLE_128B) with their 128 exponents into a ring of kTcCodeSlots; all 128 threads expand each code tile into
+// exactly the SWIZZLE_128B fp16 tile TMA would have written from the dequantized store D (common.cuh: D = fp16_rn(code·2^e)),
+// then fence.proxy.async (the wgmma reads through the async proxy) and arrive on the slot the consumers wait for.  The output
+// is therefore bit-identical to tf_tree_attn_tc over a store holding D.
 #include <string.h>
 
 #include "common.cuh"
@@ -40,6 +48,12 @@ constexpr int kTcConsumerWarps = 8;
 constexpr int kTcThreads = (kTcConsumerWarps + 1) * 32;
 constexpr uint32_t kTcTileBytes = kTcKeys * kTcD * 2;  // 32 KB: one K or V tile, also the Q block
 constexpr uint32_t kTcHalfBytes = kTcTileBytes / 2;    // one 64-element (128-byte) column half: 128 rows x 128 B
+// E4M3 store: the converter warpgroup and its ring of code tiles (16 KB of codes + 128 exponents each; 4 slots = two tiles of
+// keys ahead of the conversion, 226 KB of shared memory in all)
+constexpr int kTcConvThreads = 128;
+constexpr int kTcThreadsE4m3 = kTcConsumerWarps * 32 + kTcConvThreads;
+constexpr int kTcCodeSlots = 4;
+constexpr uint32_t kTcCodeBytes = kTcKeys * kTcD;      // 16 KB: one K or V tile of codes
 
 // ---- wgmma wrappers ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -107,6 +121,9 @@ struct TcArgs {
   float* part_m;              // [blocks][H][splits][128]   running maximum (log2 domain), -inf when the split saw nothing
   float* part_l;              // [blocks][H][splits][128]
   float* debug_s;             // nullable: scores of the CTA's first tile (block 0, head 0, split 0, rows 0..127) — test hook
+  const int8_t* k_exp;        // E4M3 store only: exponents [layer][H / grp][cap]
+  const int8_t* v_exp;
+  long long cap;
 };
 
 // Visibility of the 32 keys key0 .. key0+31 for one query row, as a bit word.  base = key0 - prefix (prefix = kv_len - tree_cols):
@@ -140,17 +157,53 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 //   accumulator element 4n + e  <->  row g + 8 (e >> 1), column 8n + 2t + (e & 1)
 //   A fragment of k-step kk     <->  {row g, keys 16kk + 2t..}, {row g+8, same}, {row g, keys 16kk + 8 + 2t..}, {row g+8, same}
 // so the scores of keys 16kk .. 16kk+15 (accumulator elements 8kk .. 8kk+7) are, packed in pairs, the A fragment of PV step kk.
-__global__ void __launch_bounds__(kTcThreads, 1)
+//
+// E4M3: converter thread ct expands 16-byte code chunk c = ct & 7 of rows 16 it + ct / 8 (it = 0..7) into the two 16-byte fp16
+// chunks 2(c & 3), 2(c & 3) + 1 of column half c / 4.  Loads and stores are whole 128-byte rows per 8-thread phase; threads with
+// c >= 4 store their second chunk first, so that each store instruction's phase also hits eight different bank groups.
+__device__ __forceinline__ void tc_convert_tile(const uint8_t* __restrict__ codes, const int8_t* __restrict__ exps, uint8_t* __restrict__ dst,
+                                                int ct) {
+#pragma unroll
+  for (int it = 0; it < kTcKeys * kTcD / 16 / kTcConvThreads; ++it) {
+    const int idx = it * kTcConvThreads + ct;
+    const int r = idx >> 3, c = idx & 7, sw = r & 7;
+    const uint4 w = *reinterpret_cast<const uint4*>(codes + r * 128 + ((c ^ sw) << 4));
+    __half fa, fb;
+    kv_e4m3_factors(exps[r], fa, fb);
+    const __half2 a2 = __half2half2(fa), b2 = __half2half2(fb);
+    const uint32_t cw[4] = {w.x, w.y, w.z, w.w};
+    uint32_t o[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const __half2 lo = kv_e4m3_apply(kv_e4m3_codes2((uint16_t)(cw[k] & 0xffffu)), a2, b2);
+      const __half2 hi = kv_e4m3_apply(kv_e4m3_codes2((uint16_t)(cw[k] >> 16)), a2, b2);
+      o[2 * k] = *reinterpret_cast<const uint32_t*>(&lo);
+      o[2 * k + 1] = *reinterpret_cast<const uint32_t*>(&hi);
+    }
+    const uint4 first = make_uint4(o[0], o[1], o[2], o[3]), second = make_uint4(o[4], o[5], o[6], o[7]);
+    uint8_t* row = dst + (c >> 2) * kTcHalfBytes + r * 128;
+    const int j0 = 2 * (c & 3);
+    const bool swap = c >= 4;
+    *reinterpret_cast<uint4*>(row + (((swap ? j0 + 1 : j0) ^ sw) << 4)) = swap ? second : first;
+    *reinterpret_cast<uint4*>(row + (((swap ? j0 : j0 + 1) ^ sw) << 4)) = swap ? first : second;
+  }
+}
+
+template <bool kE4m3>
+__global__ void __launch_bounds__(kE4m3 ? kTcThreadsE4m3 : kTcThreads, 1)
     tree_attn_tc_kernel(const __grid_constant__ CUtensorMap qmap, const __grid_constant__ CUtensorMap kmap, const __grid_constant__ CUtensorMap vmap,
                         const TcArgs a) {
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* q_s = smem;                      // [2 halves][128 rows][128 B]
   uint8_t* kv_s = q_s + kTcTileBytes;       // [slots] single tiles [2 halves][128 keys][128 B]: K0 V0 K1 V1 ...
-  uint64_t* bars = reinterpret_cast<uint64_t*>(kv_s + (size_t)kTcSlots * kTcTileBytes);
+  uint8_t* codes_s = kv_s + (size_t)kTcSlots * kTcTileBytes;  // E4M3: [code slots][128 keys][128 B], then [code slots][128] exponents
+  int8_t* cexp_s = reinterpret_cast<int8_t*>(codes_s + (size_t)kTcCodeSlots * kTcCodeBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(kE4m3 ? reinterpret_cast<uint8_t*>(cexp_s) + kTcCodeSlots * kTcKeys : codes_s);
   uint64_t* q_full = bars;                  // 1
   uint64_t* kv_full = bars + 1;             // [slots]
   uint64_t* kv_empty = kv_full + kTcSlots;  // [slots]
+  uint64_t* code_full = kv_empty + kTcSlots;  // E4M3: [code slots]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qb = blockIdx.x, h = blockIdx.y, sp = blockIdx.z;
@@ -165,12 +218,59 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < kTcSlots; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], kTcConsumerWarps); }
+    for (int s = 0; s < kTcSlots; ++s) { mbar_init(&kv_full[s], kE4m3 ? kTcConvThreads : 1); mbar_init(&kv_empty[s], kTcConsumerWarps); }
+    if constexpr (kE4m3)
+      for (int s = 0; s < kTcCodeSlots; ++s) mbar_init(&code_full[s], 1);
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (warp == kTcConsumerWarps) {
+  if constexpr (kE4m3) {
+    if (warp >= kTcConsumerWarps) {
+      // ================= converter warpgroup (thread 0 also issues the loads) =================
+      const int ct = threadIdx.x - kTcConsumerWarps * 32;
+      const int hk = h / a.grp;
+      const size_t exp_row0 = ((size_t)a.layer * (a.H / a.grp) + hk) * (size_t)a.cap;
+      // code tile i (K of key tile i / 2 for even i, V for odd i) into code slot i % kTcCodeSlots.  Its exponents stop at cap
+      // (cap and key0 are multiples of 64); a code box beyond cap is zero-filled by TMA, and a zero code is 0 at any exponent.
+      auto issue = [&](int i) {
+        const uint32_t cs = (uint32_t)i % kTcCodeSlots;
+        const int key0 = (t_begin + (i >> 1)) * kTcKeys;
+        const CUtensorMap* map = (i & 1) ? &vmap : &kmap;
+        const uint32_t ebytes = (uint32_t)min((long long)kTcKeys, a.cap - key0);
+        uint8_t* dst = codes_s + (size_t)cs * kTcCodeBytes;
+        mbar_expect_tx(&code_full[cs], kTcCodeBytes + ebytes);
+        tma_load_4d(dst, map, &code_full[cs], 0, key0, hk, a.layer);
+        tma_load_4d(dst + kTcCodeBytes / 2, map, &code_full[cs], 0, key0 + 64, hk, a.layer);
+        bulk_load(cexp_s + cs * kTcKeys, ((i & 1) ? a.v_exp : a.k_exp) + exp_row0 + key0, ebytes, &code_full[cs]);
+      };
+      if (n_tiles > 0) {
+        if (ct == 0) {
+          prefetch_tensormap(&qmap);
+          prefetch_tensormap(&kmap);
+          prefetch_tensormap(&vmap);
+          mbar_expect_tx(q_full, kTcTileBytes);
+          tc_tma_3d(smem_u32(q_s), &qmap, q_full, 0, h, qb * kTcBlockRows);
+          tc_tma_3d(smem_u32(q_s) + kTcHalfBytes, &qmap, q_full, 64, h, qb * kTcBlockRows);
+          for (int i = 0; i < min(kTcCodeSlots, 2 * n_tiles); ++i) issue(i);
+        }
+        for (int i = 0; i < 2 * n_tiles; ++i) {
+          const uint32_t cs = (uint32_t)i % kTcCodeSlots, cph = ((uint32_t)i / kTcCodeSlots) & 1u;
+          const uint32_t s = (uint32_t)i % kTcSlots, ph = ((uint32_t)i / kTcSlots) & 1u;
+          mbar_wait(&code_full[cs], cph);
+          mbar_wait(&kv_empty[s], ph ^ 1u);
+          tc_convert_tile(codes_s + (size_t)cs * kTcCodeBytes, cexp_s + cs * kTcKeys, kv_s + (size_t)s * kTcTileBytes, ct);
+          fence_proxy_async();  // the generic-proxy stores above, before the consumers' wgmma reads them through the async proxy
+          mbar_arrive(&kv_full[s]);
+          asm volatile("bar.sync 1, %0;" ::"n"(kTcConvThreads) : "memory");  // every converter thread is done with code slot cs
+          if (ct == 0 && i + kTcCodeSlots < 2 * n_tiles) issue(i + kTcCodeSlots);
+        }
+      }
+      return;
+    }
+  }
+
+  if (!kE4m3 && warp == kTcConsumerWarps) {
     // ================= TMA producer =================
     if (lane == 0 && n_tiles > 0) {
       prefetch_tensormap(&qmap);
@@ -372,9 +472,11 @@ size_t tf_tree_attn_tc_workspace_bytes(int R, int H, int kv_len_max) {
 }
 
 // q fp16 [R][H][128] contiguous; out fp16 [R][H][128]; H query heads over H / grp KV heads.  debug_scores: nullable, fp32 [128][128].
+// k_exp / v_exp non-NULL: the tensor maps are over the codes of an E4M3 store of `cap` slots (the checks on them are the caller's).
 static int tree_attn_tc_impl(const void* q, const void* k_tensormap, const void* v_tensormap, int layer, int kv_len, int R, int H,
                              int grp, int d, float scale, const uint32_t* tree_mask, int tree_cols, int causal, void* out,
-                             void* workspace, size_t workspace_bytes, float* debug_scores, tf_stream_t stream_) {
+                             void* workspace, size_t workspace_bytes, float* debug_scores, tf_stream_t stream_,
+                             const int8_t* k_exp = nullptr, const int8_t* v_exp = nullptr, long long cap = 0) {
   using namespace tf;
   cudaStream_t stream = (cudaStream_t)stream_;
   TF_CHECK_ARG(q && k_tensormap && v_tensormap && out && workspace, "tf_tree_attn_tc: NULL pointer");
@@ -427,9 +529,18 @@ static int tree_attn_tc_impl(const void* q, const void* k_tensormap, const void*
   a.part_m = a.part_o + slots * kTcBlockRows * kTcD;
   a.part_l = a.part_m + slots * kTcBlockRows;
   a.debug_s = debug_scores;
-  const size_t smem = 1024 + (size_t)(1 + kTcSlots) * kTcTileBytes + 256;
-  TF_ENSURE_DYNAMIC_SMEM(tree_attn_tc_kernel, smem);
-  tree_attn_tc_kernel<<<dim3(blocks, H, splits), kTcThreads, smem, stream>>>(qmap, kmap, vmap, a);
+  a.k_exp = k_exp;
+  a.v_exp = v_exp;
+  a.cap = cap;
+  if (k_exp != nullptr) {
+    const size_t smem = 1024 + (size_t)(1 + kTcSlots) * kTcTileBytes + (size_t)kTcCodeSlots * (kTcCodeBytes + kTcKeys) + 256;
+    TF_ENSURE_DYNAMIC_SMEM(tree_attn_tc_kernel<true>, smem);
+    tree_attn_tc_kernel<true><<<dim3(blocks, H, splits), kTcThreadsE4m3, smem, stream>>>(qmap, kmap, vmap, a);
+  } else {
+    const size_t smem = 1024 + (size_t)(1 + kTcSlots) * kTcTileBytes + 256;
+    TF_ENSURE_DYNAMIC_SMEM(tree_attn_tc_kernel<false>, smem);
+    tree_attn_tc_kernel<false><<<dim3(blocks, H, splits), kTcThreads, smem, stream>>>(qmap, kmap, vmap, a);
+  }
   TF_CHECK_LAUNCH();
   tree_attn_merge_kernel<<<dim3(R, H), 128, 0, stream>>>(a.part_o, a.part_m, a.part_l, H, R, splits, (__half*)out);
   TF_CHECK_LAUNCH();
@@ -452,6 +563,22 @@ int tf_tree_attn_tc_gqa(const void* q, const void* k_tensormap, const void* v_te
   }
   return tree_attn_tc_impl(q, k_tensormap, v_tensormap, layer, kv_len, R, Hq, Hq / Hkv, d, scale, tree_mask, tree_cols, causal, out,
                            workspace, workspace_bytes, nullptr, stream);
+}
+
+int tf_tree_attn_tc_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
+                         long long cap, int layer, int kv_len, int R, int Hq, int Hkv, int d, float scale, const uint32_t* tree_mask,
+                         int tree_cols, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0) {
+    tf::set_error("tf_tree_attn_tc_e4m3: Hq (%d) must be a positive multiple of Hkv (%d)", Hq, Hkv);
+    return TF_ERR_INVALID;
+  }
+  TF_CHECK_ARG(k_exp && v_exp, "tf_tree_attn_tc_e4m3: NULL exponent pointer");
+  TF_CHECK_ARG((((uintptr_t)k_exp | (uintptr_t)v_exp) & 15) == 0, "tf_tree_attn_tc_e4m3: exponents must be 16-byte aligned");
+  TF_CHECK_ARG(cap > 0 && cap % TF_VERIFY_BOX_KEYS == 0, "tf_tree_attn_tc_e4m3: cap (%lld) must be a positive multiple of %d", cap,
+               TF_VERIFY_BOX_KEYS);
+  TF_CHECK_ARG(kv_len <= cap, "tf_tree_attn_tc_e4m3: kv_len (%d) exceeds cap %lld", kv_len, cap);
+  return tree_attn_tc_impl(q, k_tensormap, v_tensormap, layer, kv_len, R, Hq, Hq / Hkv, d, scale, tree_mask, tree_cols, 0, out,
+                           workspace, workspace_bytes, nullptr, stream, k_exp, v_exp, cap);
 }
 
 }  // extern "C"

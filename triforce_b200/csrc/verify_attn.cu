@@ -126,12 +126,6 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
   return r;
 }
 __device__ __forceinline__ uint32_t h2u(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
-// 1-D bulk copy global -> shared completing on an mbarrier (16-byte aligned, size % 16 == 0)
-__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(smem_dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 constexpr int kPfChunk = 4096;  // bytes per L2 prefetch request (tf_verify_attn_prefetch)
 

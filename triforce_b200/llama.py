@@ -566,6 +566,15 @@ class LlamaModel:
         """`retrieval_tree_inference` of the reference (TP_llama_tree.py:406-425 → tensor_op.py:230-272): the n new tree nodes
         are written to retrieval slots [budget + storage_start, …) and attend to the whole budget plus their ancestors."""
         require_fp16_weights(self, "forward_tree_retrieval (the Sequoia tree path)")
+        return self._tree_retrieval(input_ids, graph_cache, position_ids, mask_bits, storage_start)
+
+    def forward_tree_retrieval_e4m3(self, input_ids: torch.Tensor, graph_cache, position_ids: torch.Tensor, mask_bits: torch.Tensor,
+                                    storage_start: int) -> torch.Tensor:
+        """forward_tree_retrieval for a target with E4M3 weights (fp16 weights are accepted too): forwards of <= 24 rows run on
+        tf_stream_linear_e4m3, larger ones on the one-layer D scratch (`_dense`).  The retrieval cache is fp16."""
+        return self._tree_retrieval(input_ids, graph_cache, position_ids, mask_bits, storage_start)
+
+    def _tree_retrieval(self, input_ids, graph_cache, position_ids, mask_bits, storage_start: int) -> torch.Tensor:
         Hl, d = self.local_num_heads, self.head_dim
         pos32 = position_ids.reshape(-1).to(torch.int32)
         T = graph_cache.tree_size
@@ -586,15 +595,40 @@ class LlamaModel:
         attention mask): nodes are appended at slots [seq_len, seq_len + T) and see the whole prefix plus their ancestors."""
         require_fp16_store(kv_cache, "forward_tree_verify")
         require_fp16_weights(self, "forward_tree_verify (the Sequoia tree path)")
+        return self._tree_verify(input_ids, kv_cache, position_ids, mask_bits)
+
+    def forward_tree_verify_e4m3(self, input_ids: torch.Tensor, kv_cache, position_ids: torch.Tensor,
+                                 mask_bits: torch.Tensor) -> torch.Tensor:
+        """forward_tree_verify for a target with an E4M3 full-KV store and/or E4M3 weights (fp16 ones are accepted too).  Over
+        an E4M3 store the rows are quantized on append (tf_rope_append_e4m3) and the attention runs on tf_tree_attn_tc_e4m3,
+        which computes what tf_tree_attn_tc computes on the dequantized store.  It has no other kernel, so other shapes are
+        refused."""
+        if kv_dtype_of(kv_cache) == "e4m3":
+            d, T = self.head_dim, input_ids.numel()
+            tc = os.environ.get("TRIFORCE_TREE_TC", "1")
+            if d != 128 or T == 0 or T % 128 or tc != "1":
+                raise NotImplementedError(f"tree verify over an E4M3 store runs only on the wgmma tree kernel (head_dim 128, "
+                                          f"a multiple of 128 tree rows, TRIFORCE_TREE_TC=1); got head_dim {d}, {T} rows, "
+                                          f"TRIFORCE_TREE_TC={tc}")
+        return self._tree_verify(input_ids, kv_cache, position_ids, mask_bits)
+
+    def _tree_verify(self, input_ids, kv_cache, position_ids, mask_bits) -> torch.Tensor:
         Hl, d = self.local_num_heads, self.head_dim
-        pos32 = position_ids.reshape(-1).to(torch.int32)
         T = input_ids.numel()
+        e4m3 = kv_dtype_of(kv_cache) == "e4m3"
+        pos32 = position_ids.reshape(-1).to(torch.int32)
         old_len = kv_cache.seq_len
         mask_bits = mask_bits.contiguous()
 
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
+            if e4m3:
+                st, Hkv = kv_cache.e4m3, self.local_num_kv_heads
+                ops.rope_append_e4m3(qkv, Hl, Hkv, d, self.cos, self.sin, q_out, st, l, pos_ids=pos32, slot0=old_len)
+                ops.tree_attn_tc_e4m3(q_out, st, l, old_len + T, n, Hl, Hkv, d, self.scale, mask_bits, T, out,
+                                      self._tc_workspace(n, st))
+                return out
             self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos_ids=pos32, slot0=old_len)
             self._tree_attention(q_out, kv_cache.tensor_maps, l, old_len + T, mask_bits, T, out)
             return out

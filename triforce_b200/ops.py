@@ -467,6 +467,31 @@ def tree_attn_tc_gqa(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, Hq:
     COUNTER.n += 2
 
 
+def tree_attn_tc_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float,
+                      tree_mask: Optional[torch.Tensor], tree_cols: int, out, workspace):
+    """tree_attn_tc_gqa (Hq == Hkv is MHA) over the e4m3 store (tf_tree_attn_tc_e4m3): bit-identical to tree_attn_tc over the
+    dequantized store.  No causal mode.  Workspace from tree_attn_tc_workspace(R, Hq, kv_len_max)."""
+    require_cuda(q, out, workspace)
+    _f16c(q, "q")
+    assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and store.shape[1] == Hkv
+    if tree_cols:
+        assert tree_mask is not None and tree_mask.is_contiguous() and tree_mask.element_size() == 4 and tree_mask.numel() >= R * (tree_cols // 32)
+    check(lib().tf_tree_attn_tc_e4m3(q.data_ptr(), store.k_ptr, store.v_ptr, store.k_exp.data_ptr(), store.v_exp.data_ptr(),
+                                     store.shape[2], layer, kv_len, R, Hq, Hkv, d, scale, ptr(tree_mask) if tree_cols else None,
+                                     tree_cols, out.data_ptr(), workspace.data_ptr(), workspace.numel(), stream_ptr()),
+          "tf_tree_attn_tc_e4m3")
+    COUNTER.n += 2
+
+
+def kv_compact_e4m3(store: E4m3Store, src_idx: torch.Tensor, dst_start: int):
+    """kv_compact over an e4m3 store (tf_kv_compact_e4m3): codes and exponents of rows src_idx -> dst_start.. in every (layer, head)."""
+    L, H, cap, d = store.shape
+    assert src_idx.dtype == torch.int32 and src_idx.is_cuda
+    check(lib().tf_kv_compact_e4m3(store.k_codes.data_ptr(), store.v_codes.data_ptr(), store.k_exp.data_ptr(), store.v_exp.data_ptr(),
+                                   cap, L, H, d, src_idx.data_ptr(), src_idx.numel(), dst_start, stream_ptr()), "tf_kv_compact_e4m3")
+    COUNTER.n += 1
+
+
 def kv_compact(key_store, value_store, src_idx: torch.Tensor, dst_start: int):
     """gather_kv_incremental: rows src_idx (absolute slots, int32 device tensor) -> dst_start.. in every (layer, head)."""
     L, H, cap, d = key_store.shape

@@ -56,20 +56,26 @@ def numpy_state_dict(cfg: LlamaShape, seed: int = 0, std: float | None = None, l
 
 
 def cuda_state_dict(cfg: LlamaShape, seed: int = 0, device="cuda", std: float | None = None,
-                    lm_head_std: float | None = None) -> Dict[str, torch.Tensor]:
+                    lm_head_std: float | None = None, host: bool = False) -> Dict[str, torch.Tensor]:
+    """Seeded random-init weights drawn on `device`.  host=True moves each tensor to host memory as soon as it is drawn (the same
+    values; the device holds one tensor at a time)."""
+    if host:
+        return {k: v.cpu() for k, v in _cuda_state_dict_iter(cfg, seed, device, std, lm_head_std)}
+    return dict(_cuda_state_dict_iter(cfg, seed, device, std, lm_head_std))
+
+
+def _cuda_state_dict_iter(cfg: LlamaShape, seed: int, device, std: float | None, lm_head_std: float | None):
     g = torch.Generator(device=device)
     g.manual_seed(seed)
     std = cfg.initializer_range if std is None else std
-    out = {}
     for name, shape, kind in _param_shapes(cfg):
         if kind == "ones":
-            out[name] = torch.ones(shape, dtype=torch.float16, device=device)
+            yield name, torch.ones(shape, dtype=torch.float16, device=device)
         else:
             s = lm_head_std if (lm_head_std is not None and name == "lm_head.weight") else std
             w = torch.empty(shape, dtype=torch.float16, device=device)
             w.normal_(0.0, s, generator=g)
-            out[name] = w
-    return out
+            yield name, w
 
 
 def numpy_prompt(length: int, vocab: int = 32000, seed: int = 0) -> torch.Tensor:

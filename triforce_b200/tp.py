@@ -225,16 +225,24 @@ def shard_bounds(total: int, rank: int, world: int):
 
 
 class DistributedLlama:
+    e4m3_formats = False  # SingleGpuLlama: an E4M3 full-KV store and E4M3 weights, with the E4M3 tree forwards
+
     def __init__(self, model_name_or_path: str, dtype=torch.float16, kv_offload=False, on_chip_layers=32, local_rank=0, world_size=1,
                  prefill=32768, bsz=1, gen_len=256, retrieval_budget=4096, retrieval_chunk_size=8, gamma=6, temperature=0.6,
                  top_p=0.9, ssl=0, draft=None, draft_cache=None, flash_attn=True, config: Optional[LlamaShape] = None,
                  tree_size: int = 0, kv_dtype: str = "fp16", weight_dtype: str = "fp16", retrieval_dtype: str = "fp16") -> None:
-        """`retrieval_dtype`: the rank-local retrieval cache in fp16 or E4M3 (RetrievalCache kv_dtype); the seams never see it."""
+        """`retrieval_dtype`: the rank-local retrieval cache in fp16 or E4M3 (RetrievalCache kv_dtype); the seams never see it.
+        `kv_dtype` / `weight_dtype`: the full-KV store and the target's projection weights; E4M3 only on SingleGpuLlama."""
         assert bsz == 1
-        if kv_dtype != "fp16":
+        if kv_dtype not in KV_DTYPES:
+            raise ValueError(f"kv_dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
+        if weight_dtype not in KV_DTYPES:
+            raise ValueError(f"weight_dtype must be one of {KV_DTYPES}, got {weight_dtype!r}")
+        if kv_dtype != "fp16" and not self.e4m3_formats:
             raise NotImplementedError(f"DistributedLlama (tensor parallel) keeps an fp16 full-KV store; kv_dtype={kv_dtype!r} is not supported")
-        if weight_dtype != "fp16":
+        if weight_dtype != "fp16" and not self.e4m3_formats:
             raise NotImplementedError(f"DistributedLlama (tensor parallel) keeps fp16 weights; weight_dtype={weight_dtype!r} is not supported")
+        self.kv_dtype, self.weight_dtype = kv_dtype, weight_dtype
         self.device = torch.device("cuda", local_rank)
         self.dtype = dtype
         self.local_rank, self.world_size = local_rank, world_size
@@ -259,11 +267,16 @@ class DistributedLlama:
         self.kv_cache = self.retrieval_cache = None
 
     def init_parameters(self, hf_model=None, state_dict: Optional[Dict[str, torch.Tensor]] = None, cuda_graphs: bool = True):
-        """`hf_model`: an HF LlamaForCausalLM (its state_dict is sliced for this rank, TP_layers.py:126-147)."""
+        """`hf_model`: an HF LlamaForCausalLM (its state_dict is sliced for this rank, TP_layers.py:126-147).  SingleGpuLlama with
+        E4M3 weights or an E4M3 store: pass a host state dict; the model copies one matrix at a time to the GPU, so no fp16 copy
+        of the weights is resident while the store is allocated."""
         sd = state_dict if state_dict is not None else hf_model.state_dict()
-        self.model = LlamaModel(self.config, sd, device=self.device, tp_rank=self.local_rank, tp_world=self.world_size)
+        self.model = LlamaModel(self.config, sd, device=self.device, tp_rank=self.local_rank, tp_world=self.world_size,
+                                weight_dtype=self.weight_dtype)
+        del sd
         self.num_layers = self.config.num_hidden_layers
-        self.kv_cache = FlashSimpleCache(self.model, self.prefill_len + self.gen_len + 32 + self.tree_size)  # TP_llama.py:73
+        self.kv_cache = FlashSimpleCache(self.model, self.prefill_len + self.gen_len + 32 + self.tree_size,  # TP_llama.py:73
+                                         kv_dtype=self.kv_dtype)
         budget = self.retrieval_budget if self.retrieval_budget > 0 else self.retrieval_chunk_size
         if self.tree_size > 0:
             self.retrieval_cache = RetrievalCacheSeqouia(self.model, max_budget=budget, prefill=self.prefill_len,
@@ -298,6 +311,8 @@ class DistributedLlama:
 
     @torch.inference_mode()
     def prefill(self, input_ids):
+        if self.kv_dtype == "e4m3" or self.weight_dtype == "e4m3":  # SingleGpuLlama: the layer-major prefill
+            return self.model.prefill_e4m3(input_ids, self.kv_cache)
         import math
         c = 128
         for i in range(math.ceil(input_ids.shape[1] / c)):
@@ -329,3 +344,25 @@ class DistributedLlama:
         if input_ids.shape[-1] > 64:
             return self.graph_engine.graph_draft_prefill(input_ids)
         return self.graph_engine.graph_draft_inference(input_ids, gamma_offset)
+
+
+class SingleGpuLlama(DistributedLlama):
+    """DistributedLlama on one GPU (world size 1) that also takes an E4M3 full-KV store (`kv_dtype="e4m3"`) and E4M3 projection
+    weights (`weight_dtype="e4m3"`): the prompt goes through LlamaModel.prefill_e4m3, and the Sequoia tree forwards through
+    forward_tree_retrieval_e4m3 and forward_tree_verify_e4m3.  DistributedLlama refuses both formats, because under tensor
+    parallelism its seams have no E4M3 epilogue."""
+    e4m3_formats = True
+
+    def __init__(self, model_name_or_path: str, **kw) -> None:
+        if kw.get("world_size", 1) != 1:
+            raise NotImplementedError(f"SingleGpuLlama runs on one GPU; world_size={kw['world_size']} is tensor parallel, whose "
+                                      "DistributedLlama keeps fp16 formats")
+        super().__init__(model_name_or_path, **kw)
+
+    @torch.inference_mode()
+    def retrieval_tree_inference(self, input_ids, position_ids, mask_bits, storage_start: int, storage_ids=None, attention_mask=None):
+        return self.model.forward_tree_retrieval_e4m3(input_ids, self.retrieval_cache, position_ids, mask_bits, storage_start)
+
+    @torch.inference_mode()
+    def tree_verify_inference(self, input_ids, position_ids, mask_bits):
+        return self.model.forward_tree_verify_e4m3(input_ids, self.kv_cache, position_ids, mask_bits)
