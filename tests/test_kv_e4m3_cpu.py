@@ -138,12 +138,10 @@ def test_e4m3_entry_points_check_their_arguments():
 # ---------------------------------------------------------------------------------------------------------------------
 # refusals and the switch (no device needed: every check runs before anything is allocated)
 # ---------------------------------------------------------------------------------------------------------------------
-def test_paths_without_an_e4m3_path_refuse_it():
+def test_paths_that_keep_an_fp16_store_refuse_e4m3():
     from types import SimpleNamespace
 
     from triforce_b200.cache import FlashSimpleCache, RetrievalCacheSeqouia
-    from triforce_b200.llama import LlamaModel
-    from triforce_b200.spectree import SpecTree
     from triforce_b200.tp import DistributedLlama
 
     kv = SimpleNamespace(kv_dtype="e4m3")
@@ -151,18 +149,12 @@ def test_paths_without_an_e4m3_path_refuse_it():
         FlashSimpleCache(SimpleNamespace(), 64, kv_dtype="bf16")
     with pytest.raises(NotImplementedError, match="Sequoia"):
         object.__new__(RetrievalCacheSeqouia).init_graph_cache(kv, None, 0)
-    with pytest.raises(NotImplementedError, match="SpecTree"):
-        SpecTree(SimpleNamespace(kv_cache=kv, device="cpu"))
-    with pytest.raises(NotImplementedError, match="forward_tree_verify"):
-        object.__new__(LlamaModel).forward_tree_verify(None, kv, None, None)
     with pytest.raises(NotImplementedError, match="tensor parallel"):
         DistributedLlama("llama-7B-128K", kv_dtype="e4m3")
     cache = object.__new__(FlashSimpleCache)
     cache.kv_dtype = "e4m3"
     with pytest.raises(NotImplementedError, match="update"):
         cache.update(None, None, 0)
-    with pytest.raises(NotImplementedError, match="gather_kv_incremental"):
-        cache.gather_kv_incremental([0], 0)
 
 
 def test_on_chip_takes_the_kv_dtype_switch():

@@ -57,21 +57,21 @@ def test_kv_compact_e4m3_checks_its_arguments():
     assert f(a, a, a, a, 1024, 2, 8, 128, p, 0, 5, None) == 0                                            # nothing to move
 
 
-def test_tree_verify_e4m3_refuses_other_kernels(monkeypatch):
+def test_tree_verify_over_an_e4m3_store_refuses_other_kernels(monkeypatch):
     from triforce_b200.llama import LlamaModel
 
     kv = SimpleNamespace(kv_dtype="e4m3")
     model = object.__new__(LlamaModel)
     model.local_num_heads, model.head_dim = 32, 128
     with pytest.raises(NotImplementedError, match="multiple of 128 tree rows"):
-        model.forward_tree_verify_e4m3(torch.zeros(96, dtype=torch.long), kv, None, None)
+        model.forward_tree_verify(torch.zeros(96, dtype=torch.long), kv, None, None)
     model.head_dim = 64
     with pytest.raises(NotImplementedError, match="head_dim 64"):
-        model.forward_tree_verify_e4m3(torch.zeros(512, dtype=torch.long), kv, None, None)
+        model.forward_tree_verify(torch.zeros(512, dtype=torch.long), kv, None, None)
     model.head_dim = 128
     monkeypatch.setenv("TRIFORCE_TREE_TC", "0")
     with pytest.raises(NotImplementedError, match="TRIFORCE_TREE_TC=0"):
-        model.forward_tree_verify_e4m3(torch.zeros(512, dtype=torch.long), kv, None, None)
+        model.forward_tree_verify(torch.zeros(512, dtype=torch.long), kv, None, None)
 
 
 def test_single_gpu_llama_takes_the_e4m3_formats():
@@ -86,15 +86,6 @@ def test_single_gpu_llama_takes_the_e4m3_formats():
         SingleGpuLlama("llama-13B-128K", kv_dtype="int8")
     with pytest.raises(ValueError, match="weight_dtype"):
         SingleGpuLlama("llama-13B-128K", weight_dtype="fp8")
-
-
-def test_gather_kv_incremental_e4m3_needs_an_e4m3_store():
-    from triforce_b200.cache import FlashSimpleCache
-
-    cache = object.__new__(FlashSimpleCache)
-    cache.kv_dtype = "fp16"
-    with pytest.raises(NotImplementedError, match="E4M3 full-KV store"):
-        cache.gather_kv_incremental_e4m3([0], 0)
 
 
 def test_offloading_seqouia_takes_the_dtype_switches():

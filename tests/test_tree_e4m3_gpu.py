@@ -149,13 +149,13 @@ def _tree_engine(name, kv, weights, P, B, gen_len, temperature, alpha=0.001):
 
 
 class _CompactionCheck:
-    """Wraps gather_kv_incremental_e4m3: the store rows [offset, offset + accepted) must hold exactly the accepted nodes' codes and
+    """Wraps gather_kv_incremental over an E4M3 store: the store rows [offset, offset + accepted) must hold exactly the accepted nodes' codes and
     exponents afterwards, and the retrieval tail their D."""
 
     def __init__(self, llm):
         self.llm, self.kv = llm, llm.kv_cache
-        self.orig = self.kv.gather_kv_incremental_e4m3
-        self.kv.gather_kv_incremental_e4m3 = self
+        self.orig = self.kv.gather_kv_incremental
+        self.kv.gather_kv_incremental = self
         self.checked = 0
 
     def __call__(self, indices, offset):
@@ -188,7 +188,7 @@ GREEDY = [  # (target shape, full-KV store, weights)
 
 @pytest.mark.parametrize("name,kv,weights", GREEDY, ids=[f"{a}-kv_{b}-w_{c}" for a, b, c in GREEDY])
 @torch.inference_mode()
-def test_greedy_spectree_over_e4m3_is_greedy_ar(name, kv, weights):
+def test_greedy_spectree_over_e4m3_formats_is_greedy_ar(name, kv, weights):
     P, B, rounds = 16384, 4096, 16
     llm, tsd, gm, cfg = _tree_engine(name, kv, weights, P, B, rounds * 24 + 64, 0.0)
     llm.init_parameters(state_dict=tsd, cuda_graphs=False)

@@ -131,13 +131,10 @@ def test_e4m3_weight_entry_points_check_their_arguments():
 # ---------------------------------------------------------------------------------------------------------------------
 # refusals and the switches (no device needed: every check runs before anything is allocated)
 # ---------------------------------------------------------------------------------------------------------------------
-def test_paths_without_an_e4m3_weight_path_refuse_it(monkeypatch):
-    from types import SimpleNamespace
-
+def test_paths_that_keep_fp16_weights_refuse_e4m3(monkeypatch):
     from triforce_b200.config import named_config
     from triforce_b200.hf_compat import DraftLlamaForCausalLM
     from triforce_b200.llama import LlamaModel
-    from triforce_b200.spectree import SpecTree
     from triforce_b200.synth import retune_agreement
     from triforce_b200.tp import DistributedLlama
 
@@ -158,12 +155,6 @@ def test_paths_without_an_e4m3_weight_path_refuse_it(monkeypatch):
         DistributedLlama("llama-7B-128K", weight_dtype="e4m3")
     model = object.__new__(LlamaModel)
     model.weight_dtype = "e4m3"
-    with pytest.raises(NotImplementedError, match="forward_tree_verify"):
-        model.forward_tree_verify(None, SimpleNamespace(kv_dtype="fp16"), None, None)
-    with pytest.raises(NotImplementedError, match="forward_tree_retrieval"):
-        model.forward_tree_retrieval(None, None, None, None, 0)
-    with pytest.raises(NotImplementedError, match="SpecTree"):
-        SpecTree(SimpleNamespace(kv_cache=SimpleNamespace(kv_dtype="fp16"), model=model, device="cpu"))
     with pytest.raises(NotImplementedError, match="retune_agreement"):
         retune_agreement(model, None, 0.5, 0.5, {})
 

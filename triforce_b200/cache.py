@@ -32,11 +32,27 @@ class Cache:
 
 
 class _HeadMajorStore(Cache):
-    def _alloc(self, L, H, slots, d, device):
-        self.key_store = torch.zeros((L, H, slots, d), dtype=torch.float16, device=device)
-        self.value_store = torch.zeros((L, H, slots, d), dtype=torch.float16, device=device)
+    def _alloc(self, L, H, slots, d, device, kv_dtype: str = "fp16"):
+        """K and V stores [L, H, slots, d].  kv_dtype="e4m3": the E4M3 format of include/triforce_b200.h, with one power-of-two
+        exponent per (layer, head, slot) row; `e4m3` holds codes and exponents, `key_store` / `value_store` are the uint8 codes
+        and the slot count is rounded up to a multiple of 64."""
+        self.e4m3: Optional[ops.E4m3Store] = None
+        if kv_dtype == "e4m3":
+            slots = -(-slots // ops.VERIFY_BOX_KEYS) * ops.VERIFY_BOX_KEYS
+            self.e4m3 = ops.E4m3Store.empty(L, H, slots, d, device)
+            self.key_store, self.value_store = self.e4m3.k_codes, self.e4m3.v_codes
+        else:
+            self.key_store = torch.zeros((L, H, slots, d), dtype=torch.float16, device=device)
+            self.value_store = torch.zeros((L, H, slots, d), dtype=torch.float16, device=device)
         self.layers, self.num_heads, self.head_dim, self.slots = L, H, d, slots
-        self._maps: Optional[ops.KVTensorMaps] = None
+        self._maps = self.e4m3  # an fp16 store builds its KVTensorMaps on first use
+
+    def reset(self):
+        self.key_store.zero_()
+        self.value_store.zero_()
+        if self.e4m3 is not None:
+            self.e4m3.k_exp.zero_()
+            self.e4m3.v_exp.zero_()
 
     @property
     def tensor_maps(self) -> ops.KVTensorMaps:
@@ -52,15 +68,6 @@ class _HeadMajorStore(Cache):
     @property
     def value_cache(self) -> torch.Tensor:
         return self.value_store.permute(0, 2, 1, 3).unsqueeze(1)
-
-
-class _GatherMixin:
-    def gather_kv_incremental(self, indices, offset: int):
-        """DistributedSimpleCache.gather_kv_incremental (reference cache.py:333-343): after a tree verify the KV rows of the
-        accepted nodes (`offset + i` for i in `indices`) are packed to `offset ..` in every layer; `seq_len` follows."""
-        idx = torch.tensor([int(i) + offset for i in indices], dtype=torch.int32, device=self.key_store.device)
-        ops.kv_compact(self.key_store, self.value_store, idx, offset)
-        self.seq_len = offset + len(indices)
 
 
 KV_DTYPES = ("fp16", "e4m3")
@@ -80,13 +87,11 @@ def require_fp16_store(cache, what: str) -> None:
         raise NotImplementedError(f"{what} needs an fp16 full-KV store; this one is {kv_dtype_of(cache)}")
 
 
-class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
+class FlashSimpleCache(_HeadMajorStore):
     """Full KV of the target (reference cache.py:20-61).
 
-    kv_dtype="e4m3" stores the full KV in FP8 E4M3 with one power-of-two exponent per (layer, KV head, slot) row
-    (include/triforce_b200.h): `e4m3` holds codes and exponents, `key_store` / `value_store` are the uint8 codes and the slot
-    count is rounded up to a multiple of 64.  Every kernel reading it computes what its fp16 counterpart computes on the
-    dequantized rows, so the target's numerics change with the store."""
+    kv_dtype="e4m3" stores the full KV in FP8 E4M3 (see _HeadMajorStore._alloc).  Every kernel reading it computes what its
+    fp16 counterpart computes on the dequantized rows, so the target's numerics change with the store."""
 
     def __init__(self, model, max_budget=1024, kv_dtype: str = "fp16") -> None:
         if kv_dtype not in KV_DTYPES:
@@ -96,15 +101,7 @@ class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
         self.max_budget = max_budget
         L, H, d = _model_geometry(model)
         self.hidden_size = model.config.hidden_size
-        self.e4m3: Optional[ops.E4m3Store] = None
-        if kv_dtype == "e4m3":
-            slots = -(-max_budget // ops.VERIFY_BOX_KEYS) * ops.VERIFY_BOX_KEYS
-            self.e4m3 = ops.E4m3Store.empty(L, H, slots, d, model.device)
-            self.key_store, self.value_store = self.e4m3.k_codes, self.e4m3.v_codes
-            self.layers, self.num_heads, self.head_dim, self.slots = L, H, d, slots
-            self._maps = self.e4m3
-        else:
-            self._alloc(L, H, max_budget, d, model.device)
+        self._alloc(L, H, max_budget, d, model.device, kv_dtype)
         self.seq_len_dev = torch.zeros(1, dtype=torch.int32, device=model.device)
         self._dev_mirror = 0  # value `seq_len_dev` holds once everything enqueued so far has run
         self.scores = []
@@ -114,22 +111,17 @@ class FlashSimpleCache(_HeadMajorStore, _GatherMixin):
 
     def reset(self):
         self.seq_len = 0
-        self.key_store.zero_()
-        self.value_store.zero_()
-        if self.e4m3 is not None:
-            self.e4m3.k_exp.zero_()
-            self.e4m3.v_exp.zero_()
+        super().reset()
 
     def gather_kv_incremental(self, indices, offset: int):
-        require_fp16_store(self, "gather_kv_incremental")
-        super().gather_kv_incremental(indices, offset)
-
-    def gather_kv_incremental_e4m3(self, indices, offset: int):
-        """gather_kv_incremental over an E4M3 store (tf_kv_compact_e4m3): the accepted nodes' codes and exponents, bit for bit."""
-        if kv_dtype_of(self) != "e4m3":
-            raise NotImplementedError(f"gather_kv_incremental_e4m3 needs an E4M3 full-KV store; this one is {kv_dtype_of(self)}")
+        """DistributedSimpleCache.gather_kv_incremental (reference cache.py:333-343): after a tree verify the KV rows of the
+        accepted nodes (`offset + i` for i in `indices`) are packed to `offset ..` in every layer; `seq_len` follows.  An E4M3
+        store moves the accepted nodes' codes and exponents bit for bit (tf_kv_compact_e4m3)."""
         idx = torch.tensor([int(i) + offset for i in indices], dtype=torch.int32, device=self.key_store.device)
-        ops.kv_compact_e4m3(self.e4m3, idx, offset)
+        if self.e4m3 is not None:
+            ops.kv_compact_e4m3(self.e4m3, idx, offset)
+        else:
+            ops.kv_compact(self.key_store, self.value_store, idx, offset)
         self.seq_len = offset + len(indices)
 
     def sync_seq_len_to_device(self):
@@ -163,10 +155,10 @@ class RetrievalCache(_HeadMajorStore):
     """Retrieval ("graph") cache (reference cache.py:117-198): `max_budget` slots filled with the top-k chunks of the
     full KV, followed by gamma+1 slots for the tokens being verified.
 
-    kv_dtype="e4m3" stores it in the E4M3 format of the full-KV store (include/triforce_b200.h): `e4m3` holds codes and
-    exponents, `key_store` / `value_store` are the uint8 codes and the slot count is rounded up to a multiple of 64.  The
-    build and tail copy quantize the rows of an fp16 full store, or copy the codes of an E4M3 one.  The retrieval level only
-    proposes tokens, so this changes acceptance but not the target: TriForce stays lossless with respect to the full model."""
+    kv_dtype="e4m3" stores it in the E4M3 format of the full-KV store (see _HeadMajorStore._alloc).  The build and tail copy
+    quantize the rows of an fp16 full store, or copy the codes of an E4M3 one.  The retrieval level only proposes tokens, so
+    this changes acceptance but not the target: TriForce stays lossless with respect to the full model.  Like the reference,
+    `reset` does not clear `init_graph`."""
 
     def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, gamma=6, kv_dtype: str = "fp16") -> None:
         if kv_dtype not in KV_DTYPES:
@@ -183,15 +175,7 @@ class RetrievalCache(_HeadMajorStore):
         self.real_budget = max_budget + gamma + 1
         L, H, d = _model_geometry(model)
         self.hidden_size = model.config.hidden_size
-        self.e4m3: Optional[ops.E4m3Store] = None
-        if kv_dtype == "e4m3":
-            slots = -(-self.real_budget // ops.VERIFY_BOX_KEYS) * ops.VERIFY_BOX_KEYS
-            self.e4m3 = ops.E4m3Store.empty(L, H, slots, d, model.device)
-            self.key_store, self.value_store = self.e4m3.k_codes, self.e4m3.v_codes
-            self.layers, self.num_heads, self.head_dim, self.slots = L, H, d, slots
-            self._maps = self.e4m3
-        else:
-            self._alloc(L, H, self.real_budget, d, model.device)
+        self._alloc(L, H, self.real_budget, d, model.device, kv_dtype)
         self.init_graph = False
         # last build's selection, kept for inspection / parity tests: int32 [L, H, select_sets], fp16 [L, H, chunks]
         self.topk_idx = torch.zeros((L, H, self.select_sets), dtype=torch.int32, device=model.device)
@@ -231,26 +215,22 @@ class RetrievalCache(_HeadMajorStore):
 
     def update_graph_cache(self, kv_cache: Optional[FlashSimpleCache] = None, use_device_len: bool = False, max_new: int = 0):
         """cache.py:180-182: KV of every committed generated token overwrites the budget tail, all layers."""
-        if self.e4m3 is not None:
-            if use_device_len:
-                ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, 0, kv_cache.seq_len_dev,
-                                        max_new)
-            else:
-                ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, kv_cache.seq_len)
-            return
-        if kv_dtype_of(kv_cache) == "e4m3":  # the dequantized rows of the E4M3 store
-            if use_device_len:
-                ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, 0,
-                                     kv_cache.seq_len_dev, max_new)
-            else:
-                ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, kv_cache.seq_len)
-            return
         if use_device_len:
-            ops.tail_update(kv_cache.key_store, kv_cache.value_store, self.key_store, self.value_store, self.prefill,
-                            self.max_budget, 0, kv_cache.seq_len_dev, max_new)
+            self._tail_copy(kv_cache, 0, seq_len_dev=kv_cache.seq_len_dev, max_new=max_new)
+        else:
+            self._tail_copy(kv_cache, kv_cache.seq_len)
+
+    def _tail_copy(self, kv_cache, seq_len: int, **kw):
+        """Full-KV rows [prefill, seq_len) to the budget tail in one launch: into an E4M3 cache (quantized, or the E4M3 store's
+        codes), from an E4M3 store into an fp16 cache (its dequantized rows), or fp16 to fp16.  `kw`: the device length
+        (seq_len_dev, max_new), or for the E4M3 entries a layer range (layer0, n_layers)."""
+        if self.e4m3 is not None:
+            ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, seq_len, **kw)
+        elif kv_dtype_of(kv_cache) == "e4m3":
+            ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, seq_len, **kw)
         else:
             ops.tail_update(kv_cache.key_store, kv_cache.value_store, self.key_store, self.value_store, self.prefill,
-                            self.max_budget, kv_cache.seq_len)
+                            self.max_budget, seq_len, **kw)
 
     def update(self, new_k_cache: torch.Tensor, new_v_cache: torch.Tensor, layer_idx: int):
         """Reference-compatible spec-slot write (cache.py:184-189); the engine writes them through the RoPE kernel."""
@@ -272,22 +252,11 @@ class RetrievalCache(_HeadMajorStore):
         n = seq_len - self.prefill
         if n <= 0:
             return
-        if self.e4m3 is not None:
-            ops.tail_update_to_e4m3(_full_store_of(kv_cache), self.e4m3, self.prefill, self.max_budget, seq_len, layer0=layer_idx,
-                                    n_layers=1)
-        elif kv_dtype_of(kv_cache) == "e4m3":
-            ops.tail_update_e4m3(kv_cache.e4m3, self.key_store, self.value_store, self.prefill, self.max_budget, seq_len,
-                                 layer0=layer_idx, n_layers=1)
-        else:
+        if self.e4m3 is None and kv_dtype_of(kv_cache) == "fp16":  # a slice copy: tf_tail_update has no layer range
             self.key_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.key_store[layer_idx, :, self.prefill:seq_len]
             self.value_store[layer_idx, :, self.max_budget - n:self.max_budget] = kv_cache.value_store[layer_idx, :, self.prefill:seq_len]
-
-    def reset(self):  # NB: like the reference, does not clear `init_graph`
-        self.key_store.zero_()
-        self.value_store.zero_()
-        if self.e4m3 is not None:
-            self.e4m3.k_exp.zero_()
-            self.e4m3.v_exp.zero_()
+        else:
+            self._tail_copy(kv_cache, seq_len, layer0=layer_idx, n_layers=1)
 
 
 class RetrievalCacheSeqouia(RetrievalCache):
@@ -316,8 +285,7 @@ class RetrievalCacheSeqouia(RetrievalCache):
         return self.key_cache[layer_idx], self.value_cache[layer_idx]
 
     def reset(self):
-        self.key_store.zero_()
-        self.value_store.zero_()
+        super().reset()
         self.init_graph = False  # unlike RetrievalCache.reset (cache.py:476-479)
 
 
@@ -362,8 +330,7 @@ class StreamingLLMEvictionCache(_HeadMajorStore):
         return self.key_cache[layer_idx][:, :end], self.value_cache[layer_idx][:, :end]
 
     def reset(self):
-        self.key_store.zero_()
-        self.value_store.zero_()
+        super().reset()
         if not self.strict_reference_quirks:
             self.seq_len = 0
 

@@ -44,22 +44,12 @@ class InferenceEngine:
 
     @torch.inference_mode()
     def model_run(self, input_ids: torch.LongTensor):
-        """Target forward over the FULL cache.  More than 64 ids = prompt: appended in `target_prefill_chunk`-token pieces
-        (the reference's chunking, kept because it fixes the fp16 summation order the golden logits were produced with);
-        the last call with exactly one id also builds the retrieval cache inside `LlamaModel.forward_target`
+        """Target forward over the FULL cache.  More than 64 ids = prompt: `LlamaModel.prefill` in `target_prefill_chunk`-token
+        pieces; the next call, with exactly one id, also builds the retrieval cache inside `LlamaModel.forward_target`
         (modeling_llama.py:230-238).  Up to 64 ids = a verify / decode step over the full KV (`tf_verify_attn`)."""
-        if input_ids.shape[-1] > 64 and (getattr(self.kv_cache, "kv_dtype", "fp16") == "e4m3"
-                                         or getattr(self.model, "weight_dtype", "fp16") == "e4m3"):
-            # layer-major prefill: on an E4M3 store the prompt's attention runs on an fp16 scratch layer, then the layer is
-            # quantized; E4M3 weights are dequantized once per layer instead of once per chunk
-            logits = self.model.prefill_e4m3(input_ids, self.kv_cache, chunk=self.target_prefill_chunk)
-        elif input_ids.shape[-1] > 64:  # prefill
-            c = self.target_prefill_chunk
-            for i in range(math.ceil(input_ids.shape[1] / c)):
-                logits = self.model(input_ids=input_ids[:, i * c:(i + 1) * c], kv_cache=self.kv_cache, graph_cache=None).logits
-        else:  # verification
-            logits = self.model(input_ids=input_ids, kv_cache=self.kv_cache, graph_cache=self.graph_cache).logits
-        return logits
+        if input_ids.shape[-1] > 64:  # prefill
+            return self.model.prefill(input_ids, self.kv_cache, chunk=self.target_prefill_chunk)
+        return self.model(input_ids=input_ids, kv_cache=self.kv_cache, graph_cache=self.graph_cache).logits  # verification
 
     @torch.inference_mode()
     def draft_run(self, input_ids: torch.LongTensor, gamma_offset: int = 0, probs=False, temperature=0.6, top_p=0.9):

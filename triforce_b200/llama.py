@@ -22,7 +22,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._C import lib as _C_lib
-from .cache import FlashSimpleCache, RetrievalCache, StreamingLLMEvictionCache, kv_dtype_of, require_fp16_store
+from .cache import FlashSimpleCache, RetrievalCache, StreamingLLMEvictionCache, kv_dtype_of
 from .config import LlamaShape
 from .rope import softmax_scale, tables_for
 
@@ -87,12 +87,6 @@ def shard_layer_weights(state_dict: Dict[str, torch.Tensor], config: LlamaShape,
 
 _PUSHED = object()  # a seam whose sum over ranks is still sitting in the LL inboxes (see LlamaModel._seam)
 WEIGHT_DTYPES = ("fp16", "e4m3")
-
-
-def require_fp16_weights(model, what: str) -> None:
-    """Paths without an E4M3-weight implementation refuse such a model instead of running on weights it does not hold."""
-    if getattr(model, "weight_dtype", "fp16") != "fp16":
-        raise NotImplementedError(f"{what} needs fp16 projection weights; this target stores them in {model.weight_dtype}")
 
 
 class LlamaModel:
@@ -265,6 +259,62 @@ class LlamaModel:
         else:
             ops.tree_attn_tc(q_out, maps, layer, kv_len, n, Hl, d, self.scale, mask_bits, tree_cols, out, ws, causal=causal)
 
+    # --- over a cache of either format: its `e4m3` store, or its fp16 layers through the entry points above ---------------
+    def _append(self, cache, layer, qkv, q_out, **pos):
+        """RoPE + append of the rows' K/V into `layer` of the cache (quantized into an E4M3 store); `pos`: the positions and
+        slots of rope_append."""
+        if cache.e4m3 is not None:
+            ops.rope_append_e4m3(qkv, self.local_num_heads, self.local_num_kv_heads, self.head_dim, self.cos, self.sin, q_out,
+                                 cache.e4m3, layer, **pos)
+        else:
+            self._rope_append(qkv, q_out, cache.key_store[layer], cache.value_store[layer], **pos)
+
+    def _attend_workspace(self, cache, n):
+        """The workspace `_attend` takes for n rows over the cache: the verify kernels', or None for prompt rows over an fp16
+        store."""
+        return self._workspace() if n <= ops.VERIFY_MAX_ROWS or cache.e4m3 is not None else None
+
+    def _attend(self, cache, layer, q_out, kv_len, out, ws, kv_len_dev=None, clean_keys=0, next_weights=None):
+        """Causal attention of the rows of q_out over the first kv_len keys of the cache, the rows' own keys last (see
+        ops.verify_attn for `kv_len_dev`, `clean_keys` and `next_weights`).  An E4M3 store has no L2 prefetch.  More than 32
+        rows over an fp16 store are prompt rows: they take the prefill split."""
+        n = q_out.shape[0]
+        if cache.e4m3 is not None:
+            ops.verify_attn_e4m3(q_out, cache.e4m3, layer, kv_len, n, self.local_num_heads, self.local_num_kv_heads, self.head_dim,
+                                 self.scale, out, ws, kv_len_dev=kv_len_dev, clean_keys=clean_keys)
+            return out
+        if n > ops.VERIFY_MAX_ROWS:
+            return self._prefill_attention(q_out, cache.tensor_maps, cache.key_store[layer], cache.value_store[layer], layer, kv_len,
+                                           n, out, ws)
+        self._verify_attn(q_out, cache.tensor_maps, layer, kv_len, n, out, ws, kv_len_dev=kv_len_dev, clean_keys=clean_keys,
+                          next_weights=next_weights)
+        return out
+
+    def _tree_attention(self, cache, layer, q_out, kv_len, mask_bits, tree_cols, out):
+        """Attention of the n rows of q_out over the cache's first kv_len keys, of which the last tree_cols are seen through
+        the rows' tree mask."""
+        Hl, d = self.local_num_heads, self.head_dim
+        n = q_out.shape[0]
+        if cache.e4m3 is not None:  # forward_tree_verify admits only the shapes of this kernel
+            ops.tree_attn_tc_e4m3(q_out, cache.e4m3, layer, kv_len, n, Hl, self.local_num_kv_heads, d, self.scale, mask_bits,
+                                  tree_cols, out, self._tc_workspace(n, cache.e4m3))
+            return
+        maps = cache.tensor_maps
+        if d == 128 and n >= 128 and n % 128 == 0 and os.environ.get("TRIFORCE_TREE_TC", "1") == "1":
+            # the whole tree in ONE pass over the KV on the tensor cores (wgmma, variant 2; reads each KV byte n/128 times
+            # instead of n/32 times)
+            self._tree_attn_tc(q_out, maps, layer, kv_len, n, mask_bits, tree_cols, out)
+            return
+        ws = self._workspace()
+        if self.gqa:  # blocks of VERIFY_MAX_ROWS / group-size rows (ops.verify_attn_gqa)
+            ops.verify_attn_gqa(q_out, maps, layer, kv_len, n, Hl, self.local_num_kv_heads, d, self.scale, out, ws,
+                                tree_mask=mask_bits[:n], tree_cols=tree_cols)
+            return
+        for r0 in range(0, n, ops.VERIFY_MAX_ROWS):  # blocks of <= 32 rows (tf_verify_attn_tree)
+            r1 = min(n, r0 + ops.VERIFY_MAX_ROWS)
+            ops.verify_attn_tree(q_out[r0:r1], maps, layer, kv_len, r1 - r0, Hl, d, self.scale, mask_bits[r0:r1], tree_cols,
+                                 out[r0:r1], ws)
+
     def calibrate_attention(self, kv_cache, rows: int = 7, rounds: int = 4) -> Optional[dict]:
         """Init-time load balancing of the verify attention on this GPU (tf_verify_attn_calibrate): the kernel's per-CTA key
         ranges are re-cut in proportion to the HBM rate each CTA actually gets.  `rows` <= 16 calibrates the grid of the
@@ -410,16 +460,25 @@ class LlamaModel:
             return out
         return _prefill_attention_library(q_out, key_layer, value_layer, kv_len, self.scale)
 
-    def prefill_e4m3(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128) -> torch.Tensor:
-        """Layer-major prompt prefill, for an E4M3 full-KV store and for E4M3 weights: for each layer, every `chunk`-row piece
-        runs through the layer with the ops and shapes of the chunk-major prefill (`forward_target` on `chunk` ids at a time),
-        so each layer's weights are dequantized once rather than once per piece.  On an E4M3 store the pieces append their K/V
-        to a one-layer fp16 scratch store with the fp16 RoPE kernel and attend over it with the fp16 kernels, so the prompt's
-        causal attention never reads E4M3; then the layer's rows are quantized into the store.  On an fp16 store they append
-        into, and attend over, the store's own layer.  The residual stream of all prompt rows is kept between layers; logits are
-        computed for the last piece only.  The logits and the fp16 K/V rows are therefore bit-identical to the chunk-major
-        prefill with the same capacity and the same weights."""
+    def prefill(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128) -> torch.Tensor:
+        """Prompt prefill into the full-KV store, `chunk` ids at a time; returns the logits of the last piece.
+
+        fp16 weights over an fp16 store: chunk-major, `forward_target` on each piece in turn (the reference's chunking, which
+        fixes the fp16 summation order the golden logits were produced with).
+
+        An E4M3 store or E4M3 weights: layer-major.  For each layer, every piece runs through the layer with the ops and shapes
+        of the chunk-major prefill, so each layer's weights are dequantized once rather than once per piece.  On an E4M3 store
+        the pieces append their K/V to a one-layer fp16 scratch store with the fp16 RoPE kernel and attend over it with the fp16
+        kernels, so the prompt's causal attention never reads E4M3; then the layer's rows are quantized into the store.  On an
+        fp16 store they append into, and attend over, the store's own layer.  The residual stream of all prompt rows is kept
+        between layers; logits are computed for the last piece only.  The logits and the fp16 K/V rows are therefore
+        bit-identical to the chunk-major prefill with the same capacity and the same weights."""
         e4m3_store = kv_dtype_of(kv_cache) == "e4m3"
+        if not e4m3_store and self.weight_dtype == "fp16":
+            ids = input_ids.reshape(-1)
+            for c0 in range(0, ids.numel(), chunk):
+                logits = self.forward_target(ids[c0:c0 + chunk], kv_cache)
+            return logits
         if kv_cache.seq_len != 0:
             raise NotImplementedError("the layer-major prefill starts from an empty full-KV store (reset the cache first)")
         ids = input_ids.reshape(-1)
@@ -472,62 +531,35 @@ class LlamaModel:
         Hl, d = self.local_num_heads, self.head_dim
         n = input_ids.numel()
         build = (not spec) and n == 1 and isinstance(graph_cache, RetrievalCache)
+        assert not (build and use_device_len), "a device-length forward does not build the retrieval cache"
         qs = torch.empty((len(self.layers), Hl, d), dtype=torch.float16, device=self.device) if build else None
-        ws = self._workspace() if n <= ops.VERIFY_MAX_ROWS else None
+        old_len = kv_cache.seq_len
+        if kv_dtype_of(kv_cache) == "e4m3" and not spec and n > 2 * ops.VERIFY_MAX_ROWS:
+            raise ValueError(f"a {n}-row full-KV forward over an E4M3 store: prompts go through prefill")
         if spec:
             assert n == graph_cache.gamma + 1, "retrieval verify takes exactly gamma+1 rows (cache.py:186)"
-            pos32 = position_ids.reshape(-1).to(torch.int32)
-        old_len = kv_cache.seq_len
-        e4m3 = kv_dtype_of(kv_cache) == "e4m3"
-        if e4m3 and not spec and n > 2 * ops.VERIFY_MAX_ROWS:
-            raise ValueError(f"a {n}-row full-KV forward over an E4M3 store: prompts go through prefill_e4m3")
-        if e4m3:
-            ws = self._workspace()
+            pos = dict(pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=graph_cache.max_budget)
+        elif use_device_len:
+            pos = dict(pos0_dev=kv_cache.seq_len_dev, slot0_dev=kv_cache.seq_len_dev)
+        elif position_ids is not None:
+            pos = dict(pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=old_len)
+        else:
+            pos = dict(pos0=old_len, slot0=old_len)
+        ws = self._attend_workspace(graph_cache if spec else kv_cache, n)
 
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-            if e4m3 and not spec:  # RoPE + quantized append, verify over the E4M3 store in bottom-right aligned row blocks
-                st, Hkv = kv_cache.e4m3, self.local_num_kv_heads
-                if use_device_len:
-                    kw = dict(pos0_dev=kv_cache.seq_len_dev, slot0_dev=kv_cache.seq_len_dev)
-                elif position_ids is not None:
-                    kw = dict(pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=old_len)
-                else:
-                    kw = dict(pos0=old_len, slot0=old_len)
-                ops.rope_append_e4m3(qkv, Hl, Hkv, d, self.cos, self.sin, q_out, st, l, **kw)
-                if build:
-                    qs[l] = q_out[0]
-                ops.verify_attn_e4m3(q_out, st, l, n if use_device_len else old_len + n, n, Hl, Hkv, d, self.scale, out, ws,
-                                     kv_len_dev=kv_cache.seq_len_dev if use_device_len else None)
-                return out
-            if spec and kv_dtype_of(graph_cache) == "e4m3":  # E4M3 retrieval cache: quantized append, PDL verify with the early ring fill
-                st, Hkv = graph_cache.e4m3, self.local_num_kv_heads
-                ops.rope_append_e4m3(qkv, Hl, Hkv, d, self.cos, self.sin, q_out, st, l, pos_ids=pos32, slot0=graph_cache.max_budget)
-                ops.verify_attn_e4m3(q_out, st, l, graph_cache.real_budget, n, Hl, Hkv, d, self.scale, out, ws,
-                                     clean_keys=graph_cache.max_budget)  # rope_append wrote slots >= budget only
-                return out
             if spec:
-                self._rope_append(qkv, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
-                                  slot0=graph_cache.max_budget)
-                self._verify_attn(q_out, graph_cache.tensor_maps, l, graph_cache.real_budget, n, out, ws,
-                                  clean_keys=graph_cache.max_budget,  # rope_append wrote slots >= budget only
-                                  next_weights=self.layers[l].wo if self.attn_prefetch else None)  # o_proj's weights ride into L2
-                return out
-            if use_device_len:
-                self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos0_dev=kv_cache.seq_len_dev,
-                                  slot0_dev=kv_cache.seq_len_dev)
-                self._verify_attn(q_out, kv_cache.tensor_maps, l, n, n, out, ws, kv_len_dev=kv_cache.seq_len_dev)
-                return out
-            if position_ids is not None:
-                self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l],
-                                  pos_ids=position_ids.reshape(-1).to(torch.int32), slot0=old_len)
-            else:
-                self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos0=old_len, slot0=old_len)
+                self._append(graph_cache, l, qkv, q_out, **pos)
+                return self._attend(graph_cache, l, q_out, graph_cache.real_budget, out, ws,
+                                    clean_keys=graph_cache.max_budget,  # rope_append wrote slots >= budget only
+                                    next_weights=self.layers[l].wo if self.attn_prefetch else None)  # o_proj's weights ride into L2
+            self._append(kv_cache, l, qkv, q_out, **pos)
             if build:
                 qs[l] = q_out[0]
-            return self._prefill_attention(q_out, kv_cache.tensor_maps, kv_cache.key_store[l], kv_cache.value_store[l], l,
-                                           old_len + n, n, out, ws)
+            return self._attend(kv_cache, l, q_out, n if use_device_len else old_len + n, out, ws,
+                                kv_len_dev=kv_cache.seq_len_dev if use_device_len else None)
 
         logits = self._stack(input_ids, attn_fn)
         if not spec and not use_device_len:
@@ -542,39 +574,10 @@ class LlamaModel:
         return logits.unsqueeze(0)
 
     # --- tree (Sequoia) ------------------------------------------------------------------------------------------------
-    def _tree_attention(self, q_out, maps, layer, kv_len, mask_bits, tree_cols, out):
-        """Masked attention of n rows in blocks of <= 32 rows (tf_verify_attn_tree)."""
-        Hl, d = self.local_num_heads, self.head_dim
-        n = q_out.shape[0]
-        if d == 128 and n >= 128 and n % 128 == 0 and os.environ.get("TRIFORCE_TREE_TC", "1") == "1":
-            # the whole tree in ONE pass over the KV on the tensor cores (wgmma, variant 2; reads each KV byte n/128 times
-            # instead of n/32 times)
-            self._tree_attn_tc(q_out, maps, layer, kv_len, n, mask_bits, tree_cols, out)
-            return
-        ws = self._workspace()
-        if self.gqa:  # blocks of VERIFY_MAX_ROWS / group-size rows (ops.verify_attn_gqa)
-            ops.verify_attn_gqa(q_out, maps, layer, kv_len, n, Hl, self.local_num_kv_heads, d, self.scale, out, ws,
-                                tree_mask=mask_bits[:n], tree_cols=tree_cols)
-            return
-        for r0 in range(0, n, ops.VERIFY_MAX_ROWS):
-            r1 = min(n, r0 + ops.VERIFY_MAX_ROWS)
-            ops.verify_attn_tree(q_out[r0:r1], maps, layer, kv_len, r1 - r0, Hl, d, self.scale, mask_bits[r0:r1], tree_cols,
-                                 out[r0:r1], ws)
-
     def forward_tree_retrieval(self, input_ids: torch.Tensor, graph_cache, position_ids: torch.Tensor, mask_bits: torch.Tensor,
                                storage_start: int) -> torch.Tensor:
         """`retrieval_tree_inference` of the reference (TP_llama_tree.py:406-425 → tensor_op.py:230-272): the n new tree nodes
         are written to retrieval slots [budget + storage_start, …) and attend to the whole budget plus their ancestors."""
-        require_fp16_weights(self, "forward_tree_retrieval (the Sequoia tree path)")
-        return self._tree_retrieval(input_ids, graph_cache, position_ids, mask_bits, storage_start)
-
-    def forward_tree_retrieval_e4m3(self, input_ids: torch.Tensor, graph_cache, position_ids: torch.Tensor, mask_bits: torch.Tensor,
-                                    storage_start: int) -> torch.Tensor:
-        """forward_tree_retrieval for a target with E4M3 weights (fp16 weights are accepted too): forwards of <= 24 rows run on
-        tf_stream_linear_e4m3, larger ones on the one-layer D scratch (`_dense`).  The retrieval cache is fp16."""
-        return self._tree_retrieval(input_ids, graph_cache, position_ids, mask_bits, storage_start)
-
-    def _tree_retrieval(self, input_ids, graph_cache, position_ids, mask_bits, storage_start: int) -> torch.Tensor:
         Hl, d = self.local_num_heads, self.head_dim
         pos32 = position_ids.reshape(-1).to(torch.int32)
         T = graph_cache.tree_size
@@ -583,39 +586,25 @@ class LlamaModel:
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-            self._rope_append(qkv, q_out, graph_cache.key_store[l], graph_cache.value_store[l], pos_ids=pos32,
-                              slot0=graph_cache.max_budget + storage_start)
-            self._tree_attention(q_out, graph_cache.tensor_maps, l, graph_cache.real_budget, mask_bits, T, out)
+            self._append(graph_cache, l, qkv, q_out, pos_ids=pos32, slot0=graph_cache.max_budget + storage_start)
+            self._tree_attention(graph_cache, l, q_out, graph_cache.real_budget, mask_bits, T, out)
             return out
 
         return self._stack(input_ids, attn_fn).unsqueeze(0)
 
     def forward_tree_verify(self, input_ids: torch.Tensor, kv_cache, position_ids: torch.Tensor, mask_bits: torch.Tensor) -> torch.Tensor:
         """The masked verify of all T tree nodes over the FULL KV (SpecTree_TP.py:168-175 → TP_llama_tree `inference` with an
-        attention mask): nodes are appended at slots [seq_len, seq_len + T) and see the whole prefix plus their ancestors."""
-        require_fp16_store(kv_cache, "forward_tree_verify")
-        require_fp16_weights(self, "forward_tree_verify (the Sequoia tree path)")
-        return self._tree_verify(input_ids, kv_cache, position_ids, mask_bits)
-
-    def forward_tree_verify_e4m3(self, input_ids: torch.Tensor, kv_cache, position_ids: torch.Tensor,
-                                 mask_bits: torch.Tensor) -> torch.Tensor:
-        """forward_tree_verify for a target with an E4M3 full-KV store and/or E4M3 weights (fp16 ones are accepted too).  Over
-        an E4M3 store the rows are quantized on append (tf_rope_append_e4m3) and the attention runs on tf_tree_attn_tc_e4m3,
-        which computes what tf_tree_attn_tc computes on the dequantized store.  It has no other kernel, so other shapes are
-        refused."""
+        attention mask): nodes are appended at slots [seq_len, seq_len + T) and see the whole prefix plus their ancestors.
+        Over an E4M3 store the attention runs on tf_tree_attn_tc_e4m3, which computes what tf_tree_attn_tc computes on the
+        dequantized store.  It has no other kernel, so other shapes are refused."""
+        Hl, d = self.local_num_heads, self.head_dim
+        T = input_ids.numel()
         if kv_dtype_of(kv_cache) == "e4m3":
-            d, T = self.head_dim, input_ids.numel()
             tc = os.environ.get("TRIFORCE_TREE_TC", "1")
             if d != 128 or T == 0 or T % 128 or tc != "1":
                 raise NotImplementedError(f"tree verify over an E4M3 store runs only on the wgmma tree kernel (head_dim 128, "
                                           f"a multiple of 128 tree rows, TRIFORCE_TREE_TC=1); got head_dim {d}, {T} rows, "
                                           f"TRIFORCE_TREE_TC={tc}")
-        return self._tree_verify(input_ids, kv_cache, position_ids, mask_bits)
-
-    def _tree_verify(self, input_ids, kv_cache, position_ids, mask_bits) -> torch.Tensor:
-        Hl, d = self.local_num_heads, self.head_dim
-        T = input_ids.numel()
-        e4m3 = kv_dtype_of(kv_cache) == "e4m3"
         pos32 = position_ids.reshape(-1).to(torch.int32)
         old_len = kv_cache.seq_len
         mask_bits = mask_bits.contiguous()
@@ -623,14 +612,8 @@ class LlamaModel:
         def attn_fn(l, qkv, n):
             q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
             out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-            if e4m3:
-                st, Hkv = kv_cache.e4m3, self.local_num_kv_heads
-                ops.rope_append_e4m3(qkv, Hl, Hkv, d, self.cos, self.sin, q_out, st, l, pos_ids=pos32, slot0=old_len)
-                ops.tree_attn_tc_e4m3(q_out, st, l, old_len + T, n, Hl, Hkv, d, self.scale, mask_bits, T, out,
-                                      self._tc_workspace(n, st))
-                return out
-            self._rope_append(qkv, q_out, kv_cache.key_store[l], kv_cache.value_store[l], pos_ids=pos32, slot0=old_len)
-            self._tree_attention(q_out, kv_cache.tensor_maps, l, old_len + T, mask_bits, T, out)
+            self._append(kv_cache, l, qkv, q_out, pos_ids=pos32, slot0=old_len)
+            self._tree_attention(kv_cache, l, q_out, old_len + T, mask_bits, T, out)
             return out
 
         logits = self._stack(input_ids, attn_fn)

@@ -25,7 +25,6 @@ import numpy as np
 import torch
 
 from . import ops
-from .cache import kv_dtype_of
 from .rng import TorchNoise
 from .sampling import norm_logits
 
@@ -107,12 +106,6 @@ def build_sampling(grow_map: Dict, temperature: float, device):
 class SpecTree:
     def __init__(self, engine, temperature: float = 0.6, top_p: float = 0.9, max_length=256, vocab_size=32000, grow_map=None,
                  residual_graph=None, sampling_callables=None, sample_gather_indices=None, tokenizer=None, noise=None) -> None:
-        # an E4M3 store or E4M3 weights need an engine whose tree forwards are the E4M3 ones (tp.SingleGpuLlama)
-        self.e4m3_store = kv_dtype_of(getattr(engine, "kv_cache", None)) == "e4m3"
-        e4m3_weights = getattr(getattr(engine, "model", None), "weight_dtype", "fp16") != "fp16"
-        if (self.e4m3_store or e4m3_weights) and not getattr(engine, "e4m3_formats", False):
-            raise NotImplementedError("SpecTree (the Sequoia tree path) over an E4M3 full-KV store or E4M3 weights needs an engine "
-                                      "with the E4M3 tree forwards (tp.SingleGpuLlama); this one has the fp16 ones")
         self.graph_engine = engine
         self.temperature, self.top_p = temperature, top_p
         self.residual_graph = residual_graph or get_residual
@@ -231,10 +224,7 @@ class SpecTree:
             return None, acc_count, []
         accept_tokens = self.verify_tokens[torch.tensor(accept_list, dtype=torch.long, device=self.device)]
         accept_tokens = torch.cat([accept_tokens, next_token], dim=-1)
-        if self.e4m3_store:
-            eng.kv_cache.gather_kv_incremental_e4m3(accept_list, offset)
-        else:
-            eng.kv_cache.gather_kv_incremental(accept_list, offset)
+        eng.kv_cache.gather_kv_incremental(accept_list, offset)
         eng.retrieval_cache.update_graph_cache(eng.kv_cache)
         self.draft_logits.zero_()
         self.verify_tokens.zero_()

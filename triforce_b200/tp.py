@@ -225,7 +225,7 @@ def shard_bounds(total: int, rank: int, world: int):
 
 
 class DistributedLlama:
-    e4m3_formats = False  # SingleGpuLlama: an E4M3 full-KV store and E4M3 weights, with the E4M3 tree forwards
+    e4m3_formats = False  # SingleGpuLlama: an E4M3 full-KV store and E4M3 weights
 
     def __init__(self, model_name_or_path: str, dtype=torch.float16, kv_offload=False, on_chip_layers=32, local_rank=0, world_size=1,
                  prefill=32768, bsz=1, gen_len=256, retrieval_budget=4096, retrieval_chunk_size=8, gamma=6, temperature=0.6,
@@ -311,13 +311,7 @@ class DistributedLlama:
 
     @torch.inference_mode()
     def prefill(self, input_ids):
-        if self.kv_dtype == "e4m3" or self.weight_dtype == "e4m3":  # SingleGpuLlama: the layer-major prefill
-            return self.model.prefill_e4m3(input_ids, self.kv_cache)
-        import math
-        c = 128
-        for i in range(math.ceil(input_ids.shape[1] / c)):
-            logits = self.inference(input_ids=input_ids[:, i * c:(i + 1) * c])
-        return logits
+        return self.model.prefill(input_ids, self.kv_cache)
 
     @torch.inference_mode()
     def build_retrieval_cache(self, input_ids):
@@ -348,9 +342,8 @@ class DistributedLlama:
 
 class SingleGpuLlama(DistributedLlama):
     """DistributedLlama on one GPU (world size 1) that also takes an E4M3 full-KV store (`kv_dtype="e4m3"`) and E4M3 projection
-    weights (`weight_dtype="e4m3"`): the prompt goes through LlamaModel.prefill_e4m3, and the Sequoia tree forwards through
-    forward_tree_retrieval_e4m3 and forward_tree_verify_e4m3.  DistributedLlama refuses both formats, because under tensor
-    parallelism its seams have no E4M3 epilogue."""
+    weights (`weight_dtype="e4m3"`); the model and the caches choose their kernels from the formats they hold.
+    DistributedLlama refuses both formats, because under tensor parallelism its seams have no E4M3 epilogue."""
     e4m3_formats = True
 
     def __init__(self, model_name_or_path: str, **kw) -> None:
@@ -358,11 +351,3 @@ class SingleGpuLlama(DistributedLlama):
             raise NotImplementedError(f"SingleGpuLlama runs on one GPU; world_size={kw['world_size']} is tensor parallel, whose "
                                       "DistributedLlama keeps fp16 formats")
         super().__init__(model_name_or_path, **kw)
-
-    @torch.inference_mode()
-    def retrieval_tree_inference(self, input_ids, position_ids, mask_bits, storage_start: int, storage_ids=None, attention_mask=None):
-        return self.model.forward_tree_retrieval_e4m3(input_ids, self.retrieval_cache, position_ids, mask_bits, storage_start)
-
-    @torch.inference_mode()
-    def tree_verify_inference(self, input_ids, position_ids, mask_bits):
-        return self.model.forward_tree_verify_e4m3(input_ids, self.kv_cache, position_ids, mask_bits)
