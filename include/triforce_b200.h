@@ -259,6 +259,13 @@ int tf_tree_attn_tc_gqa(const void* q, const void* k_tensormap, const void* v_te
 int tf_tree_attn_tc_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
                          long long cap, int layer, int kv_len, int R, int Hq, int Hkv, int d, float scale, const uint32_t* tree_mask,
                          int tree_cols, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream);
+/* tf_tree_attn_tc_causal_e4m3: the causal mode of tf_tree_attn_tc (causal = 1) over an E4M3 store — R >= 1 new rows whose K/V are
+ *   already in the store, over kv_len >= R keys: row i sees key j iff j <= kv_len - R + i.  The prompt rows appended after a
+ *   store's existing rows (LlamaModel.extend).  Same kernel, store arguments and checks as tf_tree_attn_tc_e4m3; the output is
+ *   bit-identical to tf_tree_attn_tc / tf_tree_attn_tc_gqa with causal = 1 over the dequantized store. */
+int tf_tree_attn_tc_causal_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp,
+                                const int8_t* v_exp, long long cap, int layer, int kv_len, int R, int Hq, int Hkv, int d, float scale,
+                                void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream);
 
 /* Init-time load balancing of tf_verify_attn (no reference counterpart; the reference has no such knob).  The kernel cuts
  * its (head, key-tile) axis into one contiguous range per CTA.  Where the SMs of a GPU do not all pull the same HBM bandwidth,

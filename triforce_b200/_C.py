@@ -79,6 +79,8 @@ _SIGNATURES = {
     "tf_kv_compact": (c_int, [c_void_p, c_void_p, c_longlong, c_longlong, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     "tf_tree_attn_tc_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_int,
                                      c_int, c_float, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tf_tree_attn_tc_causal_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_int,
+                                            c_int, c_int, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     "tf_kv_compact_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_void_p, c_int, c_int,
                                    c_void_p]),
     "tf_draft_attn": (c_int, [c_void_p, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int,

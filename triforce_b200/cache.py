@@ -160,7 +160,9 @@ class RetrievalCache(_HeadMajorStore):
     this changes acceptance but not the target: TriForce stays lossless with respect to the full model.  Like the reference,
     `reset` does not clear `init_graph`."""
 
-    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, gamma=6, kv_dtype: str = "fp16") -> None:
+    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, gamma=6, kv_dtype: str = "fp16",
+                 max_context: Optional[int] = None) -> None:
+        """`max_context` (default `prefill`): the longest context `reselect` may select from; it sizes `chunk_scores`."""
         if kv_dtype not in KV_DTYPES:
             raise ValueError(f"kv_dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
         self.kv_dtype = kv_dtype
@@ -170,8 +172,11 @@ class RetrievalCache(_HeadMajorStore):
         self.select_sets = max_budget // self.chunk_size
         self.gamma = gamma
         self.max_budget = max_budget
+        self.max_context = prefill if max_context is None else max_context
         assert prefill % self.chunk_size == 0, f"prefill should be multiple of chunk_size, got {prefill} % {self.chunk_size}"
         assert max_budget % self.chunk_size == 0, f"max_budget should be multiple of chunk_size, got {max_budget} % {self.chunk_size}"
+        if self.max_context < prefill:
+            raise ValueError(f"max_context ({self.max_context}) is below prefill ({prefill})")
         self.real_budget = max_budget + gamma + 1
         L, H, d = _model_geometry(model)
         self.hidden_size = model.config.hidden_size
@@ -179,7 +184,41 @@ class RetrievalCache(_HeadMajorStore):
         self.init_graph = False
         # last build's selection, kept for inspection / parity tests: int32 [L, H, select_sets], fp16 [L, H, chunks]
         self.topk_idx = torch.zeros((L, H, self.select_sets), dtype=torch.int32, device=model.device)
-        self.chunk_scores = torch.zeros((L, H, self.chunks), dtype=torch.float16, device=model.device)
+        self._scores = torch.zeros(L * H * (self.max_context // chunk_size), dtype=torch.float16, device=model.device)
+        self._prefill0 = prefill
+
+    def reset(self):
+        """Clears the stores and returns to the constructed `prefill` boundary (a new prompt builds there, whatever a
+        re-selection moved it to)."""
+        super().reset()
+        self.prefill, self.chunks = self._prefill0, self._prefill0 // self.chunk_size
+
+    @property
+    def chunk_scores(self) -> torch.Tensor:
+        """fp16 [L, H, chunks]: the scores of the last build, contiguous whatever the current boundary."""
+        return self._scores[:self.layers * self.num_heads * self.chunks].view(self.layers, self.num_heads, self.chunks)
+
+    def boundary(self, seq_len: int) -> int:
+        """The selection boundary `reselect` takes at a context of seq_len tokens: the last whole chunk, which must leave at
+        least the budget to select from and fit `max_context`."""
+        B = seq_len // self.chunk_size * self.chunk_size
+        if B < self.max_budget:
+            raise ValueError(f"a context of {seq_len} tokens has {B} tokens of whole chunks, fewer than the retrieval budget "
+                             f"{self.max_budget}")
+        if B > self.max_context:
+            raise ValueError(f"a context of {seq_len} tokens selects from {B} tokens, beyond max_context {self.max_context} of "
+                             f"the retrieval cache")
+        return B
+
+    def reselect(self, kv_cache: FlashSimpleCache, queries: torch.Tensor) -> int:
+        """Re-select the budget for a new question over the full KV's seq_len tokens: score the chunks below the boundary B
+        (`boundary`) with `queries` [L, Hq, d], the post-RoPE queries of the context's last token, gather the top-k, and copy
+        rows [B, seq_len) to the budget tail.  `prefill` becomes B, so later tail copies start there.  Returns B."""
+        B = self.boundary(kv_cache.seq_len)
+        self.prefill, self.chunks = B, B // self.chunk_size
+        self.build_all_layers(kv_cache, queries)
+        self._tail_copy(kv_cache, kv_cache.seq_len)
+        return B
 
     def print_status(self):
         print("[Retrieval Cache] Budget:", self.max_budget, " | PreFill:", self.prefill, " | Chunk Size:", self.chunk_size,

@@ -565,20 +565,39 @@ int tf_tree_attn_tc_gqa(const void* q, const void* k_tensormap, const void* v_te
                            workspace, workspace_bytes, nullptr, stream);
 }
 
+// The store arguments of the two E4M3 entries (the converter warpgroup's loads need them; the rest is tree_attn_tc_impl's)
+static int tree_attn_tc_e4m3_checks(const char* name, const int8_t* k_exp, const int8_t* v_exp, long long cap, int kv_len, int Hq,
+                                    int Hkv) {
+  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0) {
+    tf::set_error("%s: Hq (%d) must be a positive multiple of Hkv (%d)", name, Hq, Hkv);
+    return TF_ERR_INVALID;
+  }
+  TF_CHECK_ARG(k_exp && v_exp, "%s: NULL exponent pointer", name);
+  TF_CHECK_ARG((((uintptr_t)k_exp | (uintptr_t)v_exp) & 15) == 0, "%s: exponents must be 16-byte aligned", name);
+  TF_CHECK_ARG(cap > 0 && cap % TF_VERIFY_BOX_KEYS == 0, "%s: cap (%lld) must be a positive multiple of %d", name, cap,
+               TF_VERIFY_BOX_KEYS);
+  TF_CHECK_ARG(kv_len <= cap, "%s: kv_len (%d) exceeds cap %lld", name, kv_len, cap);
+  return TF_OK;
+}
+
 int tf_tree_attn_tc_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp, const int8_t* v_exp,
                          long long cap, int layer, int kv_len, int R, int Hq, int Hkv, int d, float scale, const uint32_t* tree_mask,
                          int tree_cols, void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
-  if (Hkv <= 0 || Hq <= 0 || Hq % Hkv != 0) {
-    tf::set_error("tf_tree_attn_tc_e4m3: Hq (%d) must be a positive multiple of Hkv (%d)", Hq, Hkv);
-    return TF_ERR_INVALID;
-  }
-  TF_CHECK_ARG(k_exp && v_exp, "tf_tree_attn_tc_e4m3: NULL exponent pointer");
-  TF_CHECK_ARG((((uintptr_t)k_exp | (uintptr_t)v_exp) & 15) == 0, "tf_tree_attn_tc_e4m3: exponents must be 16-byte aligned");
-  TF_CHECK_ARG(cap > 0 && cap % TF_VERIFY_BOX_KEYS == 0, "tf_tree_attn_tc_e4m3: cap (%lld) must be a positive multiple of %d", cap,
-               TF_VERIFY_BOX_KEYS);
-  TF_CHECK_ARG(kv_len <= cap, "tf_tree_attn_tc_e4m3: kv_len (%d) exceeds cap %lld", kv_len, cap);
+  const int rc = tree_attn_tc_e4m3_checks("tf_tree_attn_tc_e4m3", k_exp, v_exp, cap, kv_len, Hq, Hkv);
+  if (rc != TF_OK) return rc;
   return tree_attn_tc_impl(q, k_tensormap, v_tensormap, layer, kv_len, R, Hq, Hq / Hkv, d, scale, tree_mask, tree_cols, 0, out,
                            workspace, workspace_bytes, nullptr, stream, k_exp, v_exp, cap);
+}
+
+// The causal tile bound (last_key, and the split's tile count) is computed once per CTA before the roles part, so the converter
+// warpgroup loads and converts exactly the tiles the consumers read.
+int tf_tree_attn_tc_causal_e4m3(const void* q, const void* k_tensormap, const void* v_tensormap, const int8_t* k_exp,
+                                const int8_t* v_exp, long long cap, int layer, int kv_len, int R, int Hq, int Hkv, int d, float scale,
+                                void* out, void* workspace, size_t workspace_bytes, tf_stream_t stream) {
+  const int rc = tree_attn_tc_e4m3_checks("tf_tree_attn_tc_causal_e4m3", k_exp, v_exp, cap, kv_len, Hq, Hkv);
+  if (rc != TF_OK) return rc;
+  return tree_attn_tc_impl(q, k_tensormap, v_tensormap, layer, kv_len, R, Hq, Hq / Hkv, d, scale, nullptr, 0, 1, out, workspace,
+                           workspace_bytes, nullptr, stream, k_exp, v_exp, cap);
 }
 
 }  // extern "C"

@@ -131,6 +131,26 @@ def Middle_Spec(next_token, graph_engine, gamma, verbose, tokenizer, noise=None,
     return ids, buf.spec_probs[:k], acceptance_rate
 
 
+@torch.inference_mode()
+def prompt_phase(graph_engine, input_ids, trace=None, skip_target_prefill: bool = False):
+    """decoding.py:44-58: reset the three caches, prefill the target with all but the last id, run the last one (which builds
+    the retrieval cache) and prefill the draft with the whole prompt.  Returns the last id's logits."""
+    eng, ge = graph_engine.engine, graph_engine
+    if not skip_target_prefill:
+        eng.kv_cache.reset()
+    eng.graph_cache.reset()
+    eng.draft_cache.reset()
+    if not skip_target_prefill:
+        ge.inference(input_ids=input_ids[:, :-1])
+    else:  # bench.py: the prompt's KV is already in HBM from an earlier prefill; roll the length back to P-1
+        eng.kv_cache.seq_len = input_ids.shape[1] - 1
+    if trace is not None:
+        trace.append(("target_in", [int(input_ids[0, -1])]))
+    logits = ge.inference(input_ids=input_ids[:, -1:])
+    ge.graph_draft_prefill(input_ids=input_ids)
+    return logits
+
+
 class TriForceRun:
     """Step-wise form of `TriForce` (decoding.py:41-160): `prefill()` = :44-62, `step()` = one pass of the :70-141 loop.
     `TriForce(...)` below drives it; `bench.py` drives it directly to time exactly K steps."""
@@ -160,23 +180,15 @@ class TriForceRun:
 
     @torch.inference_mode()
     def prefill(self, input_ids, skip_target_prefill: bool = False):
-        eng, ge, trace = self.eng, self.ge, self.trace
-        if not skip_target_prefill:
-            eng.kv_cache.reset()
-        eng.graph_cache.reset()
-        eng.draft_cache.reset()
-        if not skip_target_prefill:
-            ge.inference(input_ids=input_ids[:, :-1])
-        else:  # bench.py: the prompt's KV is already in HBM from an earlier prefill; roll the length back to P-1
-            eng.kv_cache.seq_len = input_ids.shape[1] - 1
-        if trace is not None:
-            trace.append(("target_in", [int(input_ids[0, -1])]))
-        logits = ge.inference(input_ids=input_ids[:, -1:])
-        ge.graph_draft_prefill(input_ids=input_ids)
+        return self.start(prompt_phase(self.ge, input_ids, trace=self.trace, skip_target_prefill=skip_target_prefill))
+
+    @torch.inference_mode()
+    def start(self, logits):
+        """Sample the first token of the generation from the last row of `logits` (the prompt's, or a follow-up turn's)."""
         self.next_token = int(_sample_token(norm_logits(logits[:, -1, :], temperature=self.temperature, top_k=self.top_k,
                                                         top_p=self.top_p), self.noise, self.buf.expo).item())
-        if trace is not None:
-            trace.append(("sample", self.next_token))
+        if self.trace is not None:
+            self.trace.append(("sample", self.next_token))
         self.generated = [self.next_token]
         return self.next_token
 

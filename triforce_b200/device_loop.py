@@ -53,7 +53,10 @@ class PhiloxNoise:
         return None
 
 
-def _capture_kept(fn, mempool, warmups: int = 2):
+_WARMUPS = 2
+
+
+def _capture_kept(fn, mempool, warmups: int = _WARMUPS):
     """Warm up `fn` on a side stream, then capture it into a CUDAGraph that keeps its cudaGraph_t (not instantiated by torch)."""
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -96,6 +99,7 @@ class DeviceLoop:
         self.tokens_host = torch.zeros(g + 3, dtype=torch.int64).pin_memory()
         kv, gc, dc = eng.kv_cache, eng.graph_cache, eng.draft_cache
         max_new = min(max_new, gc.max_budget)
+        self.tail_prefill = gc.prefill  # captured into the post graph's tail copy
 
         def draft_rows(ids):  # [1, R] ids -> probabilities of all R rows (the per-offset graphs of graph_infer.py:136-150 in one)
             R = ids.shape[-1]
@@ -123,12 +127,22 @@ class DeviceLoop:
             self.res_host.copy_(self.res, non_blocking=True)
             self.tokens_host.copy_(self.tokens, non_blocking=True)
 
-        # warm-ups run the pieces eagerly: give them a consistent state, then put the caches' lengths back
+        # warm-ups run the pieces eagerly: give them a consistent state, then put back the caches' lengths and the rows the
+        # warm-ups overwrite, the draft window and the budget tail (a loop captured in the middle of a session leaves it as it was).
+        # Each warm-up of `post` advances the device length by at most gamma + 2, so its tail copy reaches at most the last
+        # (seq_len - prefill) + _WARMUPS * (gamma + 2) budget slots.
         saved_len = kv.seq_len
         kv.sync_seq_len_to_device()
         pool = graph_engine.mempool or torch.cuda.graphs.graph_pool_handle()
         rng_saved = self.rng.clone()
+        rows = min(max_new, max(0, kv.seq_len - gc.prefill) + _WARMUPS * (g + 2))
+        tail = [gc.key_store, gc.value_store] + ([gc.e4m3.k_exp, gc.e4m3.v_exp] if gc.e4m3 is not None else [])
+        tail = [t[:, :, gc.max_budget - rows:gc.max_budget] for t in tail] + [dc.key_store, dc.value_store]
+        tail_saved = [t.clone() for t in tail]
         self._graphs = [_capture_kept(pre, pool), _capture_kept(body, pool), _capture_kept(post, pool)]
+        for t, s in zip(tail, tail_saved):
+            t.copy_(s)
+        del tail_saved
         self.rng.copy_(rng_saved)
         kv.seq_len = saved_len
         kv._dev_mirror = -1
@@ -143,10 +157,15 @@ class DeviceLoop:
 
     @classmethod
     def for_engine(cls, graph_engine, gamma, temperature, top_p, eos=-1, strict_less=True, max_new=1024) -> "DeviceLoop":
-        """One captured loop per engine and sampling setup (capturing costs seconds and graph-pool memory)."""
+        """One captured loop per engine and sampling setup (capturing costs seconds and graph-pool memory).  The post graph's
+        tail copy bakes in the retrieval cache's `prefill`: after a re-selection moved it (RetrievalCache.reselect), the loop is
+        captured again."""
         key = (gamma, float(temperature), float(top_p), int(eos), bool(strict_less), int(max_new))
         cache = graph_engine.__dict__.setdefault("_device_loops", {})
-        if key not in cache:
+        loop = cache.get(key)
+        if loop is None or loop.tail_prefill != graph_engine.engine.graph_cache.prefill:
+            cache.pop(key, None)
+            del loop  # the old graphs' pool memory goes before the new capture
             cache[key] = cls(graph_engine, gamma, temperature, top_p, eos=eos, strict_less=strict_less, max_new=max_new)
         return cache[key]
 
@@ -199,7 +218,13 @@ class DeviceLoopRun:
 
     @torch.inference_mode()
     def prefill(self, input_ids, skip_target_prefill: bool = False):
-        tok = self._host.prefill(input_ids, skip_target_prefill=skip_target_prefill)
+        from .decoding import prompt_phase
+        return self.start(prompt_phase(self.ge, input_ids, skip_target_prefill=skip_target_prefill))
+
+    @torch.inference_mode()
+    def start(self, logits):
+        """Sample the first token from the last row of `logits` on the loop's noise stream and hand it to the graph."""
+        tok = self._host.start(logits)
         self.generated = [tok]
         self.next_token = tok
         kv = self.eng.kv_cache

@@ -59,15 +59,22 @@ class InferenceEngine:
         index while the keys are staged (`tf_draft_attn`).  `probs=True` returns the last row after the fused
         temperature / top-p / softmax kernel — what the draft graphs capture."""
         if input_ids.shape[-1] > 64:  # prefill
-            c = self.draft_prefill_chunk
-            for i in range(math.ceil(input_ids.shape[1] / c)):
-                self.draft_cache.evict_prefill(c)
-                logits = self.draft(input_ids=input_ids[:, i * c:(i + 1) * c], kv_cache=self.draft_cache, graph_cache=None).logits
+            logits = self.draft_prefill(input_ids)
         else:  # decoding
             logits = self.draft(input_ids=input_ids, kv_cache=self.draft_cache, graph_cache=self.draft_cache,
                                 gamma_offset=gamma_offset).logits
         if probs:
             return norm_logits(logits[0], temperature=temperature, top_k=-1, top_p=top_p)[-1]
+        return logits
+
+    @torch.inference_mode()
+    def draft_prefill(self, input_ids: torch.LongTensor):
+        """The draft's prompt path at any length: `draft_prefill_chunk`-id pieces, each after an eviction that makes room for it,
+        appended behind the window's rows (also how a follow-up turn's ids enter the window); returns the last piece's logits."""
+        c = self.draft_prefill_chunk
+        for i in range(math.ceil(input_ids.shape[1] / c)):
+            self.draft_cache.evict_prefill(c)
+            logits = self.draft(input_ids=input_ids[:, i * c:(i + 1) * c], kv_cache=self.draft_cache, graph_cache=None).logits
         return logits
 
     @torch.inference_mode()

@@ -483,14 +483,52 @@ class LlamaModel:
             raise NotImplementedError("the layer-major prefill starts from an empty full-KV store (reset the cache first)")
         ids = input_ids.reshape(-1)
         N = ids.numel()
-        L, Hkv, cap, d = kv_cache.e4m3.shape if e4m3_store else kv_cache.key_store.shape
+        cap = kv_cache.e4m3.shape[2] if e4m3_store else kv_cache.key_store.shape[2]
         if N > cap:
             raise ValueError(f"{N} prompt tokens exceed the {cap} slots of the full-KV store")
+        return self._layer_major(ids, kv_cache, chunk)
+
+    def extend(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128,
+               queries: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Append n prompt rows after the store's `seq_len` rows (a follow-up turn over a prefilled context); returns the logits
+        of the last row, [1, 1, V].  `queries`: None, or [L, H, d] fp16 that receives each layer's post-RoPE query of the last
+        row (what the retrieval cache scores chunks with, RetrievalCache.reselect).
+
+        fp16 weights over an fp16 store: `forward_target` on `chunk`-id pieces, the calls `prefill` makes, so when the existing
+        length is a multiple of `chunk`, prefill(A) then extend(B) equals prefill(A + B) bit for bit.
+        An E4M3 store or E4M3 weights: layer-major, like `prefill` (each layer's weights dequantized once per call).  Over a
+        non-empty E4M3 store each piece appends its rows with the E4M3 RoPE kernel and attends over the store: pieces of more than
+        64 rows on the causal wgmma kernel at head_dim 128 (tf_tree_attn_tc_causal_e4m3), others on the E4M3 verify attention.
+        Over an empty store the call is `prefill`."""
+        ids = input_ids.reshape(-1)
+        N, start = ids.numel(), kv_cache.seq_len
+        if N < 1:
+            raise ValueError("extend needs at least one id")
+        if start + N > kv_cache.slots:
+            raise ValueError(f"appending {N} tokens after {start} exceeds the {kv_cache.slots} slots of the full-KV store")
+        if queries is not None:
+            assert queries.dtype == torch.float16 and queries.shape == (len(self.layers), self.local_num_heads, self.head_dim)
+        if kv_dtype_of(kv_cache) == "fp16" and self.weight_dtype == "fp16":
+            for c0 in range(0, N, chunk):
+                logits = self.forward_target(ids[c0:c0 + chunk], kv_cache, queries=queries if c0 + chunk >= N else None)
+        else:
+            logits = self._layer_major(ids, kv_cache, chunk, queries)
+        return logits[:, -1:]
+
+    def _layer_major(self, ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int,
+                     queries: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The N ids after the store's seq_len rows, layer by layer in `chunk`-id pieces (see `prefill` and `extend`); the
+        caller has checked the capacity.  An empty E4M3 store takes the fp16 scratch of `prefill`."""
+        start = kv_cache.seq_len
+        e4m3_store = kv_dtype_of(kv_cache) == "e4m3"
+        scratch = e4m3_store and start == 0
+        N = ids.numel()
+        L, Hkv, cap, d = kv_cache.e4m3.shape if e4m3_store else kv_cache.key_store.shape
         Hl = self.local_num_heads
         h = self.embed_tokens[ids].contiguous()
         delta = [None] * ((N + chunk - 1) // chunk)
         x = torch.empty((min(chunk, N), h.shape[1]), dtype=torch.float16, device=self.device)
-        if e4m3_store:
+        if scratch:
             scratch_k = torch.zeros((1, Hkv, cap, d), dtype=torch.float16, device=self.device)
             scratch_v = torch.zeros_like(scratch_k)
             maps = ops.KVTensorMaps(scratch_k, scratch_v)
@@ -498,41 +536,56 @@ class LlamaModel:
             maps = kv_cache.tensor_maps
         ws = self._workspace()
         for l in range(L):
-            if e4m3_store:
+            if scratch:
                 kl, vl, ml = scratch_k[0], scratch_v[0], 0
-            else:
+            elif not e4m3_store:
                 kl, vl, ml = kv_cache.key_store[l], kv_cache.value_store[l], l
             for i, c0 in enumerate(range(0, N, chunk)):
                 c1 = min(N, c0 + chunk)
 
-                def attn_fn(_l, qkv, n, c0=c0):
+                def attn_fn(_l, qkv, n, p0=start + c0, last=c1 == N):
                     q_out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
                     out = torch.empty((n, Hl, d), dtype=torch.float16, device=self.device)
-                    self._rope_append(qkv, q_out, kl, vl, pos0=c0, slot0=c0)
-                    return self._prefill_attention(q_out, maps, kl, vl, ml, c0 + n, n, out, ws)
+                    if e4m3_store and not scratch:
+                        self._append(kv_cache, l, qkv, q_out, pos0=p0, slot0=p0)
+                        if n > 2 * ops.VERIFY_MAX_ROWS and d == 128:
+                            ops.tree_attn_tc_causal_e4m3(q_out, maps, l, p0 + n, n, Hl, Hkv, d, self.scale, out,
+                                                         self._tc_workspace(n, maps))
+                        else:
+                            self._attend(kv_cache, l, q_out, p0 + n, out, ws)
+                    else:
+                        self._rope_append(qkv, q_out, kl, vl, pos0=p0, slot0=p0)
+                        out = self._prefill_attention(q_out, maps, kl, vl, ml, p0 + n, n, out, ws)
+                    if queries is not None and last:
+                        queries[l] = q_out[-1]
+                    return out
 
                 delta[i] = self._layer(l, h[c0:c1], delta[i], x[:c1 - c0], attn_fn)
-            if e4m3_store:
+            if scratch:
                 ops.kv_quantize_e4m3(scratch_k[0], kv_cache.e4m3.k_codes[l], kv_cache.e4m3.k_exp[l], 0, N)
                 ops.kv_quantize_e4m3(scratch_v[0], kv_cache.e4m3.v_codes[l], kv_cache.e4m3.v_exp[l], 0, N)
-        if e4m3_store:
+        if scratch:
             del scratch_k, scratch_v
         del maps
         c0 = (N - 1) // chunk * chunk
         logits = self._head(h[c0:], delta[-1], x[:N - c0])
-        kv_cache.seq_len = N
+        kv_cache.seq_len = start + N
         return logits.unsqueeze(0)
 
     # --- target --------------------------------------------------------------------------------------------------------
     def forward_target(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, graph_cache: Optional[RetrievalCache] = None,
-                       position_ids: Optional[torch.Tensor] = None, spec: bool = False, use_device_len: bool = False) -> torch.Tensor:
+                       position_ids: Optional[torch.Tensor] = None, spec: bool = False, use_device_len: bool = False,
+                       queries: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Mirrors LlamaForCausalLM.forward(input_ids, kv_cache, graph_cache, position_ids, spec) of the reference.
-        `use_device_len`: take the committed length from `kv_cache.seq_len_dev` (CUDA-graph replay) instead of the int."""
+        `use_device_len`: take the committed length from `kv_cache.seq_len_dev` (CUDA-graph replay) instead of the int.
+        `queries`: None, or [L, H, d] fp16 that receives each layer's post-RoPE query of the last row (full-KV forwards)."""
         Hl, d = self.local_num_heads, self.head_dim
         n = input_ids.numel()
         build = (not spec) and n == 1 and isinstance(graph_cache, RetrievalCache)
         assert not (build and use_device_len), "a device-length forward does not build the retrieval cache"
-        qs = torch.empty((len(self.layers), Hl, d), dtype=torch.float16, device=self.device) if build else None
+        assert queries is None or not spec, "a retrieval verify does not report queries"
+        qs = queries if queries is not None else (
+            torch.empty((len(self.layers), Hl, d), dtype=torch.float16, device=self.device) if build else None)
         old_len = kv_cache.seq_len
         if kv_dtype_of(kv_cache) == "e4m3" and not spec and n > 2 * ops.VERIFY_MAX_ROWS:
             raise ValueError(f"a {n}-row full-KV forward over an E4M3 store: prompts go through prefill")
@@ -556,8 +609,8 @@ class LlamaModel:
                                     clean_keys=graph_cache.max_budget,  # rope_append wrote slots >= budget only
                                     next_weights=self.layers[l].wo if self.attn_prefetch else None)  # o_proj's weights ride into L2
             self._append(kv_cache, l, qkv, q_out, **pos)
-            if build:
-                qs[l] = q_out[0]
+            if qs is not None:
+                qs[l] = q_out[-1]
             return self._attend(kv_cache, l, q_out, n if use_device_len else old_len + n, out, ws,
                                 kv_len_dev=kv_cache.seq_len_dev if use_device_len else None)
 

@@ -470,7 +470,7 @@ def tree_attn_tc_gqa(q, maps: KVTensorMaps, layer: int, kv_len: int, R: int, Hq:
 def tree_attn_tc_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float,
                       tree_mask: Optional[torch.Tensor], tree_cols: int, out, workspace):
     """tree_attn_tc_gqa (Hq == Hkv is MHA) over the e4m3 store (tf_tree_attn_tc_e4m3): bit-identical to tree_attn_tc over the
-    dequantized store.  No causal mode.  Workspace from tree_attn_tc_workspace(R, Hq, kv_len_max)."""
+    dequantized store.  The causal mode is tree_attn_tc_causal_e4m3.  Workspace from tree_attn_tc_workspace(R, Hq, kv_len_max)."""
     require_cuda(q, out, workspace)
     _f16c(q, "q")
     assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and store.shape[1] == Hkv
@@ -480,6 +480,21 @@ def tree_attn_tc_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: 
                                      store.shape[2], layer, kv_len, R, Hq, Hkv, d, scale, ptr(tree_mask) if tree_cols else None,
                                      tree_cols, out.data_ptr(), workspace.data_ptr(), workspace.numel(), stream_ptr()),
           "tf_tree_attn_tc_e4m3")
+    COUNTER.n += 2
+
+
+def tree_attn_tc_causal_e4m3(q, store: E4m3Store, layer: int, kv_len: int, R: int, Hq: int, Hkv: int, d: int, scale: float, out,
+                             workspace):
+    """The causal mode of tree_attn_tc / tree_attn_tc_gqa over the e4m3 store (tf_tree_attn_tc_causal_e4m3): the R rows of q,
+    whose K/V are the store's last rows below kv_len, attend bottom-right causally; bit-identical to tree_attn_tc(causal=True)
+    over the dequantized store.  Workspace from tree_attn_tc_workspace(R, Hq, kv_len_max)."""
+    require_cuda(q, out, workspace)
+    _f16c(q, "q")
+    assert q.is_contiguous() and out.is_contiguous() and q.shape[-3:] == (R, Hq, d) and store.shape[1] == Hkv
+    check(lib().tf_tree_attn_tc_causal_e4m3(q.data_ptr(), store.k_ptr, store.v_ptr, store.k_exp.data_ptr(), store.v_exp.data_ptr(),
+                                            store.shape[2], layer, kv_len, R, Hq, Hkv, d, scale, out.data_ptr(), workspace.data_ptr(),
+                                            workspace.numel(), stream_ptr()),
+          "tf_tree_attn_tc_causal_e4m3")
     COUNTER.n += 2
 
 
