@@ -1,20 +1,21 @@
-"""The device Philox stream of the whole-loop graph, restated on the CPU (csrc/loop_graph.cu).
+"""The device Philox stream of the whole-loop graph, restated on the CPU (csrc/spec_decisions.cuh, used by csrc/loop_graph.cu).
 
-    philox4x32_10       loop_graph.cu:35-46   Random123's Philox4x32-10: ten rounds of two 32x32->64 multiplies
-                                              (M0 = 0xD2511F53 on c0, M1 = 0xCD9E8D57 on c2), output
-                                              (hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0), key bumped by (0x9E3779B9, 0xBB67AE85)
-                                              after every round
-    element layout      loop_graph.cu:47-49   element i of draw `draw` of stream `seed` is lane i % 4 of
-                                              Philox(counter = (i / 4, draw_lo, draw_hi, 0), key = (seed_lo, seed_hi));
-                        loop_graph.cu:73-78   loop_sample walks the same layout one counter (four elements) at a time
-    word -> uniform     philox_to_uniform     u = (float32(x >> 8) + 0.5f) * 2^-24, float32 round-to-nearest-even.  Above
-                                              2^23 the sum is a tie and rounds to even, so x >> 8 == 0xFFFFFF lands on 1.0
-                                              (`uniform_current`).  The kernel maps that single 1.0 to 1 - 2^-24
-                                              (0x3f7fffff), a value the sum never produces (`uniform`); every other word
-                                              keeps its bits
-    exponential         philox_exponential    -logf(u) in float32 (CUDA's logf, within 1 ulp); `exponential` gives the
-                                              float64 value the device result is compared with
-    one draw            philox_fill_kernel    element i < n of draw `state[1]`; state[1] += 1 per fill
+    philox4x32_10       spec_decisions.cuh:71-82    Random123's Philox4x32-10: ten rounds of two 32x32->64 multiplies
+                                                    (M0 = 0xD2511F53 on c0, M1 = 0xCD9E8D57 on c2), output
+                                                    (hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0), key bumped by
+                                                    (0x9E3779B9, 0xBB67AE85) after every round
+    element layout      spec_decisions.cuh:90-93    element i of draw `draw` of stream `seed` is lane i % 4 of
+                                                    Philox(counter = (i / 4, draw_lo, draw_hi, 0), key = (seed_lo, seed_hi));
+                        spec_decisions.cuh:134-141  the sampler's Philox source (ExpoFromPhilox) walks the same layout one
+                                                    counter (four elements) at a time
+    word -> uniform     philox_to_uniform           u = (float32(x >> 8) + 0.5f) * 2^-24, float32 round-to-nearest-even.  Above
+                                                    2^23 the sum is a tie and rounds to even, so x >> 8 == 0xFFFFFF lands on 1.0
+                                                    (`uniform_current`).  The kernel maps that single 1.0 to 1 - 2^-24
+                                                    (0x3f7fffff), a value the sum never produces (`uniform`); every other word
+                                                    keeps its bits
+    exponential         philox_exponential          -logf(u) in float32 (CUDA's logf, within 1 ulp); `exponential` gives the
+                                                    float64 value the device result is compared with
+    one draw            philox_fill_kernel          element i < n of draw `state[1]`; state[1] += 1 per fill
 """
 from __future__ import annotations
 

@@ -273,16 +273,21 @@ __global__ void __launch_bounds__(256) tail_update_to_e4m3_kernel(const void* __
   }
 }
 
+// StreamingLLM window slide (cache.py:263-265 evict_for_spec): rows [src, src + n_rows) → [dst_start, …) of every (layer, head),
+// K and V, with src = src_start + *shift_dev, or src_start when shift_dev is NULL (the device loop reads its shift from device
+// memory)
 __global__ void __launch_bounds__(256) window_slide_kernel(__half* __restrict__ K, __half* __restrict__ V, long long ls,
-                                                           long long hs, int D, int src_start, int dst_start, int n_rows) {
+                                                           long long hs, int D, int src_start, const int32_t* __restrict__ shift_dev,
+                                                           int dst_start, int n_rows) {
   extern __shared__ __align__(16) uint8_t wsm[];
   uint4* buf = reinterpret_cast<uint4*>(wsm);
   const int h = blockIdx.x, layer = blockIdx.y;
+  const int src_row = src_start + (shift_dev ? *shift_dev : 0);
   const int nvec = n_rows * D / 8;
   __half* bases[2] = {K + (size_t)layer * ls + (size_t)h * hs, V + (size_t)layer * ls + (size_t)h * hs};
 #pragma unroll
   for (int w = 0; w < 2; ++w) {
-    const uint4* src = reinterpret_cast<const uint4*>(bases[w] + (size_t)src_start * D);
+    const uint4* src = reinterpret_cast<const uint4*>(bases[w] + (size_t)src_row * D);
     uint4* dst = reinterpret_cast<uint4*>(bases[w] + (size_t)dst_start * D);
     for (int i = threadIdx.x; i < nvec; i += blockDim.x) buf[i] = src[i];  // clone semantics: read everything first
     __syncthreads();
@@ -619,7 +624,20 @@ int tf_window_slide(void* K, void* V, long long layer_stride, long long head_str
   TF_ENSURE_DYNAMIC_SMEM(window_slide_kernel, 200 * 1024);
   dim3 grid(H, n_layers);
   window_slide_kernel<<<grid, 256, smem, (cudaStream_t)stream_>>>((__half*)K, (__half*)V, layer_stride, head_stride, d, src_start,
-                                                                  dst_start, n_rows);
+                                                                  nullptr, dst_start, n_rows);
+  TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_window_slide_dev(void* K, void* V, long long layer_stride, long long head_stride, int L, int H, int d, int src_base,
+                        const int32_t* shift_dev, int dst_start, int n_rows, tf_stream_t stream) {
+  using namespace tf;
+  TF_CHECK_ARG(K && V && shift_dev && L >= 1 && H >= 1 && n_rows >= 1 && d % 8 == 0, "tf_window_slide_dev: bad arguments");
+  const size_t smem = (size_t)n_rows * d * 2;
+  TF_CHECK_SUPPORTED(smem <= 200 * 1024, "tf_window_slide_dev: window of %d rows does not fit in shared memory", n_rows);
+  TF_ENSURE_DYNAMIC_SMEM(window_slide_kernel, 200 * 1024);
+  window_slide_kernel<<<dim3(H, L), 256, smem, (cudaStream_t)stream>>>((__half*)K, (__half*)V, layer_stride, head_stride, d, src_base,
+                                                                      shift_dev, dst_start, n_rows);
   TF_CHECK_LAUNCH();
   return TF_OK;
 }

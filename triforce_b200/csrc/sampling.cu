@@ -1,13 +1,13 @@
 // Sampling kernels: temperature + top-p + softmax (utils/sampling.py:5-60), multinomial-as-argmax (:63-65),
-// residual max_fn (:68-75) and the fused speculative accept/reject walks of utils/decoding.py:97-134,192-220.
+// residual max_fn (:68-75) and the fused speculative accept/reject walks of utils/decoding.py:97-134,192-220 for the step-wise
+// loop, whose noise comes from buffers.  The sampler and the speculative decisions are spec_decisions.cuh's, shared with the
+// device loop (loop_graph.cu).
 // One CTA per logits row; everything a row needs lives in shared memory (32768 floats = 128 KB).
 #include <float.h>
 
-#include "common.cuh"
+#include "spec_decisions.cuh"
 
 namespace tf {
-
-constexpr int kThreads = 1024;
 
 // ---- block-wide primitives (1024 threads) ---------------------------------------------------------------------------
 __device__ __forceinline__ float block_reduce_max(float v, float* red) {
@@ -17,15 +17,6 @@ __device__ __forceinline__ float block_reduce_max(float v, float* red) {
   __syncthreads();
   float r = (threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : -INFINITY;
   r = warp_max(r);
-  return r;
-}
-__device__ __forceinline__ float block_reduce_sum(float v, float* red) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : 0.f;
-  r = warp_sum(r);
   return r;
 }
 __device__ __forceinline__ int block_reduce_sum_int(int v, int* red) {
@@ -77,37 +68,6 @@ __device__ __forceinline__ T block_exclusive_scan(T v, T* red /* [32] */) {
   return red[warp] + inc - v;
 }
 
-struct ArgBest {
-  float v;
-  int i;
-};
-__device__ __forceinline__ bool arg_better(float v, int i, float bv, int bi) {
-  // torch.argmax: NaN counts as the maximum; first index on ties
-  const bool vn = v != v, bn = bv != bv;
-  if (vn != bn) return vn;
-  if (vn && bn) return i < bi;
-  return v > bv || (v == bv && i < bi);
-}
-__device__ __forceinline__ ArgBest block_argmax(ArgBest b, float* redv, int* redi) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, b.v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, b.i, o);
-    if (arg_better(ov, oi, b.v, b.i)) { b.v = ov; b.i = oi; }
-  }
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) { redv[threadIdx.x >> 5] = b.v; redi[threadIdx.x >> 5] = b.i; }
-  __syncthreads();
-  ArgBest r{redv[threadIdx.x & 31], redi[threadIdx.x & 31]};
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, r.v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, r.i, o);
-    if (arg_better(ov, oi, r.v, r.i)) { r.v = ov; r.i = oi; }
-  }
-  return r;
-}
-
 // torch.argmax of row[0, V); every thread returns the winner.  Eight independent loads in flight per thread.
 __device__ __forceinline__ int block_row_argmax(const float* __restrict__ row, int V, float* redv, int* redi) {
   ArgBest b{-INFINITY, 0x7fffffff};
@@ -130,29 +90,6 @@ __device__ __forceinline__ int block_row_argmax(const float* __restrict__ row, i
 // special-case path of div.rn at every unrolled call site, which would bloat the 25 K-instruction norm_logits body and stall
 // it on instruction fetch.
 __device__ __noinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-
-// argmax_i num(i) / expo[i] over [0,V); every thread returns the winner.  Eight independent iterations in flight per thread.
-template <typename F>
-__device__ __forceinline__ int block_sample(F num, const float* __restrict__ expo, int V, float* redv, int* redi) {
-  ArgBest b{-INFINITY, 0x7fffffff};
-  const int step = blockDim.x;
-  int i = threadIdx.x;
-  for (; i + 7 * step < V; i += 8 * step) {
-    float n[8], e[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) { n[u] = num(i + u * step); e[u] = expo[i + u * step]; }
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const float v = __fdiv_rn(n[u], e[u]);
-      if (arg_better(v, i + u * step, b.v, b.i)) { b.v = v; b.i = i + u * step; }
-    }
-  }
-  for (; i < V; i += step) {
-    const float v = __fdiv_rn(num(i), expo[i]);
-    if (arg_better(v, i, b.v, b.i)) { b.v = v; b.i = i; }
-  }
-  return block_argmax(b, redv, redi).i;
-}
 
 // --------------------------------------------------------------------------------------------------------------------
 // norm_logits (temperature, top-p, softmax) — sort-free and deterministic.
@@ -355,7 +292,7 @@ __global__ void __launch_bounds__(kThreads) sample_argmax_kernel(const float* __
   __shared__ int redi[32];
   const float* p = probs + (size_t)blockIdx.x * ps;
   const float* e = expo + (size_t)blockIdx.x * es;
-  const int t = block_sample([&](int i) { return p[i]; }, e, V, redv, redi);
+  const int t = block_sample([&](int i) { return p[i]; }, ExpoFromBuffer{e}, V, redv, redi);
   if (threadIdx.x == 0) out[blockIdx.x] = (int64_t)t;
 }
 
@@ -375,15 +312,8 @@ __global__ void __launch_bounds__(kThreads) residual_probs_kernel(const float* _
 }
 
 // --------------------------------------------------------------------------------------------------------------------
-// fused speculative decisions
+// fused speculative decisions (spec_decisions.cuh) over uniforms and exponentials read from buffers
 // --------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool accept_test(float r, float p, float q, bool strict_less) {
-  const float ratio = __fdiv_rn(p, q);
-  if (ratio != ratio) return false;  // torch.min propagates NaN → comparison is False
-  const float m = fminf(1.f, ratio);
-  return strict_less ? (r < m) : (r <= m);
-}
-
 __global__ void __launch_bounds__(kThreads) middle_accept_kernel(const float* __restrict__ sp, const float* __restrict__ vp,
                                                                  int64_t* __restrict__ verify_tokens,
                                                                  const float* __restrict__ uniform,
@@ -392,45 +322,7 @@ __global__ void __launch_bounds__(kThreads) middle_accept_kernel(const float* __
                                                                  float* __restrict__ spec_probs) {
   __shared__ float redv[32];
   __shared__ int redi[32];
-  const int n = st[0];
-  const int k = st[1];
-  const int64_t t = verify_tokens[n + 1];
-  const float* vpn = vp + (size_t)n * V;
-  const bool accept = accept_test(uniform[0], vpn[t], sp[t], true);
-  const int row = accept ? n + 1 : n;
-  const float* vrow = vp + (size_t)row * V;
-  const int t2 = block_sample([&](int i) { return vrow[i]; }, expo, V, redv, redi);  // contains __syncthreads
-  // proposal rows attributed to the emitted ids (decoding.py:194,202 / :213)
-  float* d0 = spec_probs + (size_t)k * V;
-  if ((V & 3) == 0) {  // rows are 16-byte aligned (V * 4 B per row on top of 256-byte-aligned allocations)
-    const float4* s0 = reinterpret_cast<const float4*>(vpn);
-    float4* t0 = reinterpret_cast<float4*>(d0);
-    for (int i = threadIdx.x; i < V / 4; i += kThreads) t0[i] = s0[i];
-    if (accept) {
-      const float4* s1 = reinterpret_cast<const float4*>(vrow);
-      float4* t1 = reinterpret_cast<float4*>(spec_probs + (size_t)(k + 1) * V);
-      for (int i = threadIdx.x; i < V / 4; i += kThreads) t1[i] = s1[i];
-    }
-  } else {
-    for (int i = threadIdx.x; i < V; i += kThreads) d0[i] = vpn[i];
-    if (accept) {
-      float* d1 = spec_probs + (size_t)(k + 1) * V;
-      for (int i = threadIdx.x; i < V; i += kThreads) d1[i] = vrow[i];
-    }
-  }
-  if (threadIdx.x == 0) {
-    int nn, kk;
-    if (accept) {
-      out_ids[k] = t;
-      out_ids[k + 1] = (int64_t)t2;
-      nn = n + 2; kk = k + 2;
-    } else {
-      out_ids[k] = (int64_t)t2;
-      nn = n + 1; kk = k + 1;
-    }
-    if (nn <= gamma) verify_tokens[nn] = (int64_t)t2;
-    st[0] = nn; st[1] = kk; st[2] = accept ? 1 : 0; st[3] += accept ? 1 : 0; st[4] += 1;
-  }
+  middle_spec_decision(sp, vp, verify_tokens, uniform[0], ExpoFromBuffer{expo}, gamma, V, st, out_ids, spec_probs, redv, redi);
 }
 
 __global__ void verify_accept_kernel(const float* __restrict__ p_rows, const float* __restrict__ q_rows,
@@ -438,22 +330,9 @@ __global__ void verify_accept_kernel(const float* __restrict__ p_rows, const flo
                                      int strict_less, int64_t eos, int64_t first_token, int32_t* __restrict__ res,
                                      int64_t* __restrict__ pass_tokens) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  int count = 0, rejected = 0, examined = 0, hit_eos = 0;
-  pass_tokens[0] = first_token;
-  for (int i = 1; i < g2 + 2; ++i) pass_tokens[i] = 100;  // decoding.py:94
-  for (int i = 0; i < g2; ++i) {
-    const int64_t t = gen[i];
-    ++examined;
-    if (accept_test(uniforms[i], p_rows[(size_t)i * V + t], q_rows[(size_t)i * V + t], strict_less != 0)) {
-      ++count;
-      pass_tokens[count] = t;
-      if (t == eos) { hit_eos = 1; break; }
-    } else {
-      rejected = 1;
-      break;
-    }
-  }
-  res[0] = count; res[1] = rejected; res[2] = examined; res[3] = hit_eos;
+  const AcceptWalk w = accept_walk(p_rows, q_rows, gen, g2, [&](int i) { return uniforms[i]; }, V, strict_less != 0, eos,
+                                   first_token, pass_tokens, g2 + 2);
+  res[0] = w.count; res[1] = w.rejected; res[2] = w.examined; res[3] = w.hit_eos;
 }
 
 __global__ void __launch_bounds__(kThreads) verify_resample_kernel(const float* __restrict__ p_rows,
@@ -466,25 +345,12 @@ __global__ void __launch_bounds__(kThreads) verify_resample_kernel(const float* 
   __shared__ int redi[32];
   const int count = res[0];
   const int rejected = res[1];
-  __syncthreads();
-  if (rejected) {
-    const float* p = p_rows + (size_t)count * V;
-    const float* q = q_rows + (size_t)count * V;
-    float s = 0.f;
-    for (int i = threadIdx.x; i < V; i += kThreads) {
-      const float x = p[i] - q[i];
-      s += x > 0.f ? x : 0.f;
-    }
-    const float S = block_reduce_sum(s, redv);
-    const int t = block_sample([&](int i) { const float x = p[i] - q[i]; return __fdiv_rn(x > 0.f ? x : 0.f, S); },
-                               expo, V, redv, redi);
-    if (threadIdx.x == 0) { out_token[0] = t; pass_tokens[count + 1] = t; }
-  } else if (count == g2) {
-    const float* p = p_rows + (size_t)g2 * V;
-    const int t = block_sample([&](int i) { return p[i]; }, expo, V, redv, redi);
-    if (threadIdx.x == 0) { out_token[0] = t; pass_tokens[count + 1] = t; res[0] = count + 1; }
-  } else {
-    if (threadIdx.x == 0) out_token[0] = gen[count - 1];  // stopped on an accepted EOS: nothing is drawn
+  __syncthreads();  // every thread has read res[0] before thread 0 rewrites it
+  const int64_t next = resample_after_walk(p_rows, q_rows, gen, g2, count, rejected != 0, ExpoFromBuffer{expo}, V, pass_tokens,
+                                           redv, redi);
+  if (threadIdx.x == 0) {
+    out_token[0] = next;
+    if (!rejected && count == g2) res[0] = count + 1;
   }
 }
 
