@@ -20,7 +20,7 @@ import kv_e4m3_oracle as eo
 from attn_needles import report_time_and_memory  # noqa: F401  (autouse fixture: wall time and peak memory per test)
 from e2e_util import TokenizerStub
 from test_model_production_gpu import production_model
-from test_sampling_loop_gpu import _chi2, _chi2_threshold
+from chi2_util import chi2, chi2_threshold
 from test_tp_gpu import _run
 from triforce_b200.cache import FlashSimpleCache, RetrievalCache, StreamingLLMEvictionCache
 from triforce_b200.config import named_config
@@ -206,9 +206,9 @@ def test_first_emitted_token_is_distributed_as_the_target():
         r, toks = loop.read()
         counts[toks[0]] += 1
     assert counts[p == 0].sum() == 0, np.flatnonzero((p == 0) & (counts > 0))[:10]
-    stat, df = _chi2(counts, p)
-    stat_c, df_c = _chi2(counts, p_t1)
-    print(f"\n[lossless, e4m3 retrieval cache] {N} launches: chi2 vs p {stat:.1f} (df {df}, 1e-6 threshold {_chi2_threshold(df):.1f}); "
-          f"vs p at temperature 1 {stat_c:.1f} (df {df_c}, threshold {_chi2_threshold(df_c):.1f})")
-    assert stat < _chi2_threshold(df)
-    assert stat_c > _chi2_threshold(df_c)
+    stat, df = chi2(counts, p)
+    stat_c, df_c = chi2(counts, p_t1)
+    print(f"\n[lossless, e4m3 retrieval cache] {N} launches: chi2 vs p {stat:.1f} (df {df}, 1e-6 threshold {chi2_threshold(df):.1f}); "
+          f"vs p at temperature 1 {stat_c:.1f} (df {df_c}, threshold {chi2_threshold(df_c):.1f})")
+    assert stat < chi2_threshold(df)
+    assert stat_c > chi2_threshold(df_c)

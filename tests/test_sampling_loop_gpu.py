@@ -16,6 +16,7 @@ import pytest
 import torch
 
 import philox_oracle as px
+from chi2_util import chi2, chi2_threshold
 from oracle import triforce_oracle as orc
 from triforce_b200 import ops
 
@@ -377,35 +378,6 @@ def test_loop_verify_matches_oracle(V):
 # ---------------------------------------------------------------------------------------------------------------------
 # (d) speculative sampling is lossless
 # ---------------------------------------------------------------------------------------------------------------------
-Z_1E6 = 4.753424308822899  # standard normal quantile at 1 - 10^-6
-
-
-def _chi2_threshold(df: int) -> float:
-    """Upper 10^-6 quantile of chi-square(df), Wilson-Hilferty."""
-    a = 2.0 / (9.0 * df)
-    return df * (1.0 - a + Z_1E6 * np.sqrt(a)) ** 3
-
-
-def _chi2(counts: np.ndarray, probs: np.ndarray):
-    """Pearson statistic over the bins with probs > 0, pooled in ascending expected count to >= 5 each; returns (stat, df)."""
-    N = counts.sum()
-    pos = np.flatnonzero(probs > 0)
-    exp = N * probs[pos].astype(np.float64)
-    cnt = counts[pos].astype(np.float64)
-    order = np.argsort(exp, kind="stable")
-    ce, cc = np.cumsum(exp[order]), np.cumsum(cnt[order])
-    cut, last = [], 0.0
-    for i, v in enumerate(ce):
-        if v - last >= 5:
-            cut.append(i)
-            last = v
-    if cut[-1] != len(ce) - 1:
-        cut[-1] = len(ce) - 1  # fold an under-filled tail into the last bin
-    be = np.diff(np.concatenate([[0.0], ce[cut]]))
-    bc = np.diff(np.concatenate([[0.0], cc[cut]]))
-    return float(((bc - be) ** 2 / be).sum()), len(be) - 1
-
-
 def _rows(V: int):
     rng = np.random.Generator(np.random.PCG64(V))
     if V == 1000:
@@ -480,16 +452,16 @@ def test_speculative_sampling_is_lossless(V, g2):
     counts = _first_token_counts(p, q, g2, N)
     assert counts.sum() == N
     assert counts[p == 0].sum() == 0, np.flatnonzero((p == 0) & (counts > 0))[:10]
-    stat, df = _chi2(counts, p)
-    thr = _chi2_threshold(df)
-    stat_q, df_q = _chi2(counts, q)
+    stat, df = chi2(counts, p)
+    thr = chi2_threshold(df)
+    stat_q, df_q = chi2(counts, q)
     a, b = np.argsort(-p, kind="stable")[:2]
     p2 = p.astype(np.float64)
     p2[a] -= 0.02
     p2[b] += 0.02
-    stat_2, df_2 = _chi2(counts, p2)
+    stat_2, df_2 = chi2(counts, p2)
     print(f"\n[lossless] V {V} g2 {g2}: chi2 vs p {stat:.1f} (df {df}, 1e-6 threshold {thr:.1f}); vs q {stat_q:.1f} "
-          f"(threshold {_chi2_threshold(df_q):.1f}); vs p with 2% moved {stat_2:.1f} (threshold {_chi2_threshold(df_2):.1f})")
+          f"(threshold {chi2_threshold(df_q):.1f}); vs p with 2% moved {stat_2:.1f} (threshold {chi2_threshold(df_2):.1f})")
     assert stat < thr
-    assert stat_q > _chi2_threshold(df_q)
-    assert stat_2 > _chi2_threshold(df_2)
+    assert stat_q > chi2_threshold(df_q)
+    assert stat_2 > chi2_threshold(df_2)
