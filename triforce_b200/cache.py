@@ -302,11 +302,14 @@ class RetrievalCacheSeqouia(RetrievalCache):
     """DistributedRetrievalCache_Seqouia (reference cache.py:385-483): the retrieval budget followed by `tree_size` slots
     for the nodes of the speculation tree (instead of gamma+1 slots)."""
 
-    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, tree_size=128, kv_dtype: str = "fp16") -> None:
+    def __init__(self, model, max_budget=1024, prefill=1024, chunk_size=8, tree_size=128, kv_dtype: str = "fp16",
+                 max_context: Optional[int] = None) -> None:
+        """`max_context`: as in RetrievalCache (the longest context `reselect` may select from; default `prefill`)."""
         if kv_dtype != "fp16":
             raise NotImplementedError(f"the Sequoia tree path keeps an fp16 retrieval cache (its tree growth needs a tree mode the "
                                       f"e4m3 verify attention does not have); kv_dtype={kv_dtype!r} is not supported")
-        super().__init__(model, max_budget=max_budget, prefill=prefill, chunk_size=chunk_size, gamma=tree_size - 1)
+        super().__init__(model, max_budget=max_budget, prefill=prefill, chunk_size=chunk_size, gamma=tree_size - 1,
+                         max_context=max_context)
         self.tree_size = tree_size
         assert self.real_budget == max_budget + tree_size
 

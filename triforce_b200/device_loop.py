@@ -43,6 +43,13 @@ class PhiloxNoise:
     def uniform_into(self, out: torch.Tensor) -> torch.Tensor:
         return ops.philox_fill(self.state, 0, out)
 
+    def tree_uniform_into(self, out: torch.Tensor) -> torch.Tensor:
+        """The race noise of a Sequoia tree's growth (`SpecTree.rand`, fp32): ONE draw, element i = the uniform of element i of
+        the flattened buffer.  The uniforms lie strictly inside (0, 1), so `log(u) / q` is finite or -inf, never NaN."""
+        if out.dtype != torch.float32:
+            raise ValueError(f"PhiloxNoise draws fp32 race noise; the buffer is {out.dtype} (SpecTree(race_dtype=torch.float32))")
+        return ops.philox_fill(self.state, 0, out)
+
     def mark(self):
         return None
 

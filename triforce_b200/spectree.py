@@ -105,13 +105,16 @@ def build_sampling(grow_map: Dict, temperature: float, device):
 
 class SpecTree:
     def __init__(self, engine, temperature: float = 0.6, top_p: float = 0.9, max_length=256, vocab_size=32000, grow_map=None,
-                 residual_graph=None, sampling_callables=None, sample_gather_indices=None, tokenizer=None, noise=None) -> None:
+                 residual_graph=None, sampling_callables=None, sample_gather_indices=None, tokenizer=None, noise=None,
+                 race_dtype=torch.float16) -> None:
+        """`race_dtype`: the uniform race noise `self.rand` of the growth, fp16 like the reference's buffer (SpecTree_TP.py:86)
+        or fp32 (what session.TreeSession uses: fp16 uniforms bias the race, DESIGN.md section 7)."""
         self.graph_engine = engine
         self.temperature, self.top_p = temperature, top_p
         self.residual_graph = residual_graph or get_residual
         self.tokenizer = tokenizer
         self.device = engine.device
-        self.dtype = torch.float16
+        self.dtype = race_dtype
         self.grow_map = grow_map or load_grow_map("512")
         if sampling_callables is None:
             sampling_callables, sample_gather_indices = build_sampling(self.grow_map, temperature, self.device)

@@ -230,9 +230,12 @@ class DistributedLlama:
     def __init__(self, model_name_or_path: str, dtype=torch.float16, kv_offload=False, on_chip_layers=32, local_rank=0, world_size=1,
                  prefill=32768, bsz=1, gen_len=256, retrieval_budget=4096, retrieval_chunk_size=8, gamma=6, temperature=0.6,
                  top_p=0.9, ssl=0, draft=None, draft_cache=None, flash_attn=True, config: Optional[LlamaShape] = None,
-                 tree_size: int = 0, kv_dtype: str = "fp16", weight_dtype: str = "fp16", retrieval_dtype: str = "fp16") -> None:
+                 tree_size: int = 0, kv_dtype: str = "fp16", weight_dtype: str = "fp16", retrieval_dtype: str = "fp16",
+                 max_context: Optional[int] = None) -> None:
         """`retrieval_dtype`: the rank-local retrieval cache in fp16 or E4M3 (RetrievalCache kv_dtype); the seams never see it.
-        `kv_dtype` / `weight_dtype`: the full-KV store and the target's projection weights; E4M3 only on SingleGpuLlama."""
+        `kv_dtype` / `weight_dtype`: the full-KV store and the target's projection weights; E4M3 only on SingleGpuLlama.
+        `max_context` (default `prefill`): the longest context follow-up turns may grow to (session.TreeSession): the full-KV
+        store holds max_context + gen_len + 32 + tree_size rows, and the retrieval cache may re-select up to it."""
         assert bsz == 1
         if kv_dtype not in KV_DTYPES:
             raise ValueError(f"kv_dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
@@ -250,6 +253,9 @@ class DistributedLlama:
         self.config = config or named_config(_NAME_TO_SHAPE.get(model_name_or_path, model_name_or_path))
         self.vocab_size = self.config.vocab_size
         self.prefill_len, self.gen_len = prefill, gen_len
+        self.max_context = prefill if max_context is None else max_context
+        if self.max_context < prefill:
+            raise ValueError(f"max_context ({self.max_context}) is below prefill ({prefill})")
         self.retrieval_budget, self.retrieval_chunk_size = retrieval_budget, retrieval_chunk_size
         self.temperature, self.top_p, self.gamma = temperature, top_p, gamma
         self.draft, self.draft_cache = draft, draft_cache
@@ -275,17 +281,17 @@ class DistributedLlama:
                                 weight_dtype=self.weight_dtype)
         del sd
         self.num_layers = self.config.num_hidden_layers
-        self.kv_cache = FlashSimpleCache(self.model, self.prefill_len + self.gen_len + 32 + self.tree_size,  # TP_llama.py:73
+        self.kv_cache = FlashSimpleCache(self.model, self.max_context + self.gen_len + 32 + self.tree_size,  # TP_llama.py:73
                                          kv_dtype=self.kv_dtype)
         budget = self.retrieval_budget if self.retrieval_budget > 0 else self.retrieval_chunk_size
         if self.tree_size > 0:
             self.retrieval_cache = RetrievalCacheSeqouia(self.model, max_budget=budget, prefill=self.prefill_len,
                                                          chunk_size=self.retrieval_chunk_size, tree_size=self.tree_size,
-                                                         kv_dtype=self.retrieval_dtype)
+                                                         kv_dtype=self.retrieval_dtype, max_context=self.max_context)
         else:
             self.retrieval_cache = RetrievalCache(self.model, max_budget=budget, prefill=self.prefill_len,
                                                   chunk_size=self.retrieval_chunk_size, gamma=self.gamma,
-                                                  kv_dtype=self.retrieval_dtype)
+                                                  kv_dtype=self.retrieval_dtype, max_context=self.max_context)
         if self.draft is not None:
             self.graph_engine = GraphInferenceEngine(self.model, self.kv_cache, self.retrieval_cache, self.draft, self.draft_cache)
             self.graph_engine.engine.draft_prefill_chunk = 128  # TP_llama.py:118-126
