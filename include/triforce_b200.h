@@ -45,7 +45,8 @@ int tf_sm_count(void);
  * start while their predecessor on the stream drains (barrier setup, descriptor and weight prefetch) and execute
  * griddepcontrol.wait before touching its outputs.  Process-wide bit mask, default 0 (off); graph-capturable:
  * 1 add_rmsnorm, 2 silu_mul, 4 rope_append, 8 draft_attn, 16 verify_attn, 32 skinny_gemm, 64 skinny_gemm pulls its weight rows
- * towards L2 before it waits, 128 stream_linear (weight ring filled before it waits), 256 allreduce_oneshot (lets the next projection prefetch during the exchange). */
+ * towards L2 before it waits, 128 stream_linear (weight ring filled before it waits), 256 allreduce_oneshot (lets the next projection prefetch during the exchange),
+ * 512 token_logprobs. */
 int tf_set_pdl(int mask);
 
 /* 128-byte TMA descriptor (CUtensorMap) over a head-major fp16 KV tensor [layers][heads][cap][d]; written to
@@ -511,6 +512,16 @@ int tf_norm_logits(const float* logits, long long row_stride, int rows, int V, f
 int tf_sample_argmax(const float* probs, long long probs_row_stride, const float* expo, long long expo_row_stride,
                      int rows, int V, int64_t* out_tokens, tf_stream_t stream);
 int tf_residual_probs(const float* p, const float* q, int V, float* out, tf_stream_t stream);
+/* tf_token_logprobs: the score of a given continuation under the model's own (T = 1) distribution.  For each of `rows` fp32
+ *   logits rows x (row r at logits + r * row_stride, V entries) and the int32 id t = ids[r]:
+ *     logprob[r] = x[t] - logsumexp(x)   (fp32; the max-shifted sum of exp in fp32),
+ *     argmax[r]  = the first maximal index, torch.argmax's rule (NaN counts as maximal), as tf_norm_logits at T = 0.
+ *   One CTA per row streams the row from global memory once, so V is not bounded by TF_SAMPLING_MAX_VOCAB.  The reduction
+ *   order is fixed: two launches give the same bits.  Graph-capturable; PDL (tf_set_pdl bit 512): waits for its
+ *   predecessor before reading the logits.  The ids must lie in [0, V); the kernel does not check them (the caller does,
+ *   on the host).  NULL pointers, rows < 0, V < 1 and row_stride < V are TF_ERR_INVALID; rows == 0 launches nothing. */
+int tf_token_logprobs(const float* logits, long long row_stride, int rows, int V, const int32_t* ids, float* logprob,
+                      int32_t* argmax, tf_stream_t stream);
 
 /* ---- fused speculative accept/reject (one warp-level walk + one CTA-wide resample) -----------------------------
  * tf_middle_accept: one inner (`Middle_Spec`) decision, utils/decoding.py:192-220.

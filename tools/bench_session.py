@@ -8,6 +8,9 @@ top_p 0.9, T 0.6, TriForce through the whole-loop device graph (triforce_b200.se
 A leg times the fresh prefill, turn 1, then follow-ups of 64, 256 and 1024 tokens.  A follow-up is split into extend, re-selection,
 draft feed and the re-capture of the whole-loop graph; its time to first token runs from the start of append to the first
 sampled token.  ms per outer step is the host time of each graph launch and read-back after --warmup steps of the turn.
+After each follow-up's turn, `Session.score` of the follow-up's ids is timed twice (`score_first_ms`, `score_ms`): it forwards
+the pending token and those ids, the rows the append's extend forwarded, and rolls the store back, so the next follow-up starts
+from the same state.  The append's own fields are timed before any score, as without scoring.
 
 Prints one JSON line with the card's name, power limit and max SM clock beside the numbers.
 
@@ -72,7 +75,8 @@ def leg(a) -> dict:
     if fmt == "fp16":
         retune_agreement(target, draft, 0.003, 0.003, {})
     torch.cuda.empty_cache()
-    slots = P + sum(FOLLOW_UPS) + 8 * (a.gen + 2 * GAMMA)
+    # room for the scores after each follow-up too: the pending token and the largest follow-up's ids
+    slots = P + sum(FOLLOW_UPS) + max(FOLLOW_UPS) + 1 + 8 * (a.gen + 2 * GAMMA)
     cache = FlashSimpleCache(target, slots, kv_dtype=fmt)
     graph_cache = RetrievalCache(target, max_budget=BUDGET, prefill=P, gamma=GAMMA, chunk_size=CHUNK, kv_dtype=fmt,
                                  max_context=slots // CHUNK * CHUNK)
@@ -117,9 +121,17 @@ def leg(a) -> dict:
             s.append(ids[off:off + n])
             off += n
             log, t2 = turn(100 + n)
+            score_ms = []
+            for _ in range(2):
+                torch.cuda.synchronize()
+                t1 = time.perf_counter()
+                s.score(ids[off - n:off])
+                torch.cuda.synchronize()
+                score_ms.append(1e3 * (time.perf_counter() - t1))
             end_first = next(e for tag, _, e in log if tag == "first_token")
             parts = {tag: 1e3 * sum(x for t, x, _ in log if t == tag) for tag in ("extend", "reselect", "draft_feed", "capture")}
             out[f"follow_up_{n}"] = {**{f"{k}_ms": v for k, v in parts.items()}, "first_token_ms": 1e3 * (end_first - t0),
+                                     "score_first_ms": score_ms[0], "score_ms": score_ms[1],
                                      "turn": t2, "boundary": graph_cache.prefill, "length": s.length}
         out["peak_gib"] = torch.cuda.max_memory_allocated() / 2 ** 30
     return out

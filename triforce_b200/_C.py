@@ -132,6 +132,7 @@ _SIGNATURES = {
     "tf_norm_logits": (c_int, [c_void_p, c_longlong, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
     "tf_sample_argmax": (c_int, [c_void_p, c_longlong, c_void_p, c_longlong, c_int, c_int, c_void_p, c_void_p]),
     "tf_residual_probs": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "tf_token_logprobs": (c_int, [c_void_p, c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "tf_tree_accept_walk": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
     "tf_middle_accept": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
@@ -143,7 +144,7 @@ _SIGNATURES = {
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
-DEFAULT_PDL_MASK = 1 | 2 | 4 | 8 | 16 | 32 | 128 | 256
+DEFAULT_PDL_MASK = 1 | 2 | 4 | 8 | 16 | 32 | 128 | 256 | 512
 
 
 class TriForceNativeError(RuntimeError):
@@ -166,7 +167,7 @@ def lib() -> ctypes.CDLL:
         fn.argtypes = args
     _lib = L
     # programmatic dependent launch mask of the decode-path kernels (tf_set_pdl): on by default for every kernel of the chain
-    # (1 add_rmsnorm, 2 silu_mul, 4 rope_append, 8 draft_attn, 16 verify_attn on short stores, 32 skinny_gemm, 128 stream_linear, 256 the one-shot peer all-reduce);
+    # (1 add_rmsnorm, 2 silu_mul, 4 rope_append, 8 draft_attn, 16 verify_attn on short stores, 32 skinny_gemm, 128 stream_linear, 256 the one-shot peer all-reduce, 512 token_logprobs);
     L.tf_set_pdl(int(os.environ.get("TRIFORCE_PDL", str(DEFAULT_PDL_MASK))))
     return L
 

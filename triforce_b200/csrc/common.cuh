@@ -55,7 +55,7 @@ void set_error(const char* fmt, ...);
 
 int sm_count();
 // tf_set_pdl() mask: which decode-path kernels are launched with programmatic stream serialization
-enum PdlBit { kPdlNorm = 1, kPdlSilu = 2, kPdlRope = 4, kPdlDraftAttn = 8, kPdlVerifyAttn = 16, kPdlSkinny = 32, kPdlSkinnyPrefetch = 64, kPdlStream = 128, kPdlAllReduce = 256 };
+enum PdlBit { kPdlNorm = 1, kPdlSilu = 2, kPdlRope = 4, kPdlDraftAttn = 8, kPdlVerifyAttn = 16, kPdlSkinny = 32, kPdlSkinnyPrefetch = 64, kPdlStream = 128, kPdlAllReduce = 256, kPdlLogprobs = 512 };
 bool pdl_enabled(int bit);
 
 // Launch with (optionally) the programmatic-dependent-launch attribute: the kernel may start while its predecessor on the

@@ -296,6 +296,71 @@ __global__ void __launch_bounds__(kThreads) sample_argmax_kernel(const float* __
   if (threadIdx.x == 0) out[blockIdx.x] = (int64_t)t;
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// token_logprobs: log p(ids[r] | row r) = x[t] - logsumexp(x) and torch.argmax of each fp32 logits row.  One CTA streams its
+// row once: every thread keeps a running (max m, sum s of exp(x - m)) and an ArgBest over the elements {tid + 1024 j}, eight
+// loads in flight, then the block merges the pairs in a fixed butterfly.  Fixed element-to-thread assignment and merge order:
+// two launches give the same bits.  No shared row buffer, so V is not limited by TF_SAMPLING_MAX_VOCAB.
+// --------------------------------------------------------------------------------------------------------------------
+// s (a sum of exp(x - m)) re-expressed against the new maximum M >= m; an empty sum (m == -inf) stays as it is
+__device__ __forceinline__ float lse_rescale(float s, float m, float M) { return m == M ? s : s * expf(m - M); }
+__device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os) {
+  const float M = fmaxf(m, om);
+  s = lse_rescale(s, m, M) + lse_rescale(os, om, M);  // commutative: both lanes of a butterfly pair compute the same bits
+  m = M;
+}
+
+__global__ void __launch_bounds__(kThreads) token_logprobs_kernel(const float* __restrict__ logits, long long row_stride, int V,
+                                                                  const int32_t* __restrict__ ids, float* __restrict__ logprob,
+                                                                  int32_t* __restrict__ argmax) {
+  __shared__ float redm[32], reds[32], redv[32];
+  __shared__ int redi[32];
+  pdl_launch_dependents();
+  pdl_wait();  // the logits come from the predecessor
+  const float* row = logits + (size_t)blockIdx.x * row_stride;
+  float m = -INFINITY, s = 0.f;
+  ArgBest b{-INFINITY, 0x7fffffff};
+  const int step = blockDim.x;
+  int i = threadIdx.x;
+  for (; i + 7 * step < V; i += 8 * step) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v[u] = row[i + u * step];
+    float cm = m;
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      cm = fmaxf(cm, v[u]);
+      if (arg_better(v[u], i + u * step, b.v, b.i)) { b.v = v[u]; b.i = i + u * step; }
+    }
+    s = lse_rescale(s, m, cm);
+    m = cm;
+#pragma unroll
+    for (int u = 0; u < 8; ++u) s += v[u] == -INFINITY ? 0.f : expf(v[u] - m);  // NaN propagates into s
+  }
+  for (; i < V; i += step) {
+    const float v = row[i];
+    if (arg_better(v, i, b.v, b.i)) { b.v = v; b.i = i; }
+    const float cm = fmaxf(m, v);
+    s = lse_rescale(s, m, cm);
+    m = cm;
+    s += v == -INFINITY ? 0.f : expf(v - m);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) lse_merge(m, s, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, s, o));
+  if ((threadIdx.x & 31) == 0) { redm[threadIdx.x >> 5] = m; reds[threadIdx.x >> 5] = s; }
+  const int win = block_argmax(b, redv, redi).i;  // its barriers also publish redm / reds
+  if (threadIdx.x >= 32) return;
+  m = redm[threadIdx.x];
+  s = reds[threadIdx.x];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) lse_merge(m, s, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, s, o));
+  if (threadIdx.x == 0) {
+    const float xt = row[ids[blockIdx.x]];
+    logprob[blockIdx.x] = (xt - m) - logf(s);
+    argmax[blockIdx.x] = win;
+  }
+}
+
 __global__ void __launch_bounds__(kThreads) residual_probs_kernel(const float* __restrict__ p, const float* __restrict__ q,
                                                                   int V, float* __restrict__ out) {
   __shared__ float redf[32];
@@ -502,6 +567,18 @@ int tf_sample_argmax(const float* probs, long long probs_row_stride, const float
   sample_argmax_kernel<<<rows, kThreads, 0, (cudaStream_t)stream_>>>(probs, probs_row_stride, expo, expo_row_stride, V,
                                                                      out_tokens);
   TF_CHECK_LAUNCH();
+  return TF_OK;
+}
+
+int tf_token_logprobs(const float* logits, long long row_stride, int rows, int V, const int32_t* ids, float* logprob,
+                      int32_t* argmax, tf_stream_t stream_) {
+  using namespace tf;
+  TF_CHECK_ARG(logits && ids && logprob && argmax, "tf_token_logprobs: NULL pointer");
+  TF_CHECK_ARG(rows >= 0 && V >= 1 && row_stride >= V, "tf_token_logprobs: bad rows %d / V %d / row stride %lld", rows, V,
+               row_stride);
+  if (rows == 0) return TF_OK;
+  TF_CHECK_CUDA(launch_kernel(kPdlLogprobs, token_logprobs_kernel, dim3(rows), dim3(kThreads), 0, (cudaStream_t)stream_, logits,
+                              row_stride, V, ids, logprob, argmax));
   return TF_OK;
 }
 

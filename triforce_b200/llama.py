@@ -460,8 +460,43 @@ class LlamaModel:
             return out
         return _prefill_attention_library(q_out, key_layer, value_layer, kv_len, self.scale)
 
-    def prefill(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128) -> torch.Tensor:
+    def _score_targets(self, ids: torch.Tensor, logprobs) -> Optional[torch.Tensor]:
+        """The int32 ids[1:] that `logprobs` (fp32 [N-1], int32 [N-1]) receives the scores of, checked once for the whole call;
+        None without `logprobs`."""
+        if logprobs is None:
+            return None
+        lp, am = logprobs
+        n = ids.numel() - 1
+        here = lambda t: t.device.type == self.device.type and self.device.index in (None, t.device.index)  # "cuda" is cuda:k
+        if lp.dtype != torch.float32 or am.dtype != torch.int32 or lp.shape != (n,) or am.shape != (n,) or not here(lp) \
+                or not here(am):
+            raise ValueError(f"logprobs is a (float32 [{n}], int32 [{n}]) pair on {self.device} for {n + 1} ids")
+        targets = ids[1:].to(torch.int32)
+        if n:
+            lo, hi = (int(v) for v in torch.aminmax(targets))
+            V = self.config.vocab_size
+            if lo < 0 or hi >= V:
+                raise ValueError(f"token ids must lie in [0, {V}); got ids in [{lo}, {hi}]")
+        return targets
+
+    @staticmethod
+    def _score_piece(logits: torch.Tensor, c0: int, targets: Optional[torch.Tensor], logprobs) -> None:
+        """Scores of the piece of rows starting at prompt row c0 (its logits [rows, V]): row c0 + j is scored against
+        targets[c0 + j] = ids[c0 + j + 1], so a piece's last row takes the next piece's first id, and the prompt's last row
+        (which has no next id) none."""
+        if targets is None:
+            return
+        r = min(logits.shape[0], targets.numel() - c0)
+        if r > 0:
+            lp, am = logprobs
+            ops.token_logprobs(logits[:r], targets[c0:c0 + r], lp[c0:c0 + r], am[c0:c0 + r], check_ids=False)
+
+    def prefill(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128, logprobs=None) -> torch.Tensor:
         """Prompt prefill into the full-KV store, `chunk` ids at a time; returns the logits of the last piece.
+
+        `logprobs`: None, or a (float32 [N-1], int32 [N-1]) pair on the model's device that receives, for i < N-1, log p(ids[i+1] |
+        ids[:i+1]) under the model's own distribution and the argmax of row i (ops.token_logprobs), reduced piece by piece as
+        the prompt runs.  The returned logits, the store's rows and its length are the same with and without it.
 
         fp16 weights over an fp16 store: chunk-major, `forward_target` on each piece in turn (the reference's chunking, which
         fixes the fp16 summation order the golden logits were produced with).
@@ -472,24 +507,26 @@ class LlamaModel:
         kernels, so the prompt's causal attention never reads E4M3; then the layer's rows are quantized into the store.  On an
         fp16 store they append into, and attend over, the store's own layer.  The residual stream of all prompt rows is kept
         between layers; logits are computed for the last piece only.  The logits and the fp16 K/V rows are therefore
-        bit-identical to the chunk-major prefill with the same capacity and the same weights."""
+        bit-identical to the chunk-major prefill with the same capacity and the same weights.  With `logprobs` the head also runs
+        on every other piece, one piece at a time after the last layer (E4M3 weights: lm_head dequantized once)."""
         e4m3_store = kv_dtype_of(kv_cache) == "e4m3"
+        ids = input_ids.reshape(-1)
+        targets = self._score_targets(ids, logprobs)
         if not e4m3_store and self.weight_dtype == "fp16":
-            ids = input_ids.reshape(-1)
             for c0 in range(0, ids.numel(), chunk):
                 logits = self.forward_target(ids[c0:c0 + chunk], kv_cache)
+                self._score_piece(logits[0], c0, targets, logprobs)
             return logits
         if kv_cache.seq_len != 0:
             raise NotImplementedError("the layer-major prefill starts from an empty full-KV store (reset the cache first)")
-        ids = input_ids.reshape(-1)
         N = ids.numel()
         cap = kv_cache.e4m3.shape[2] if e4m3_store else kv_cache.key_store.shape[2]
         if N > cap:
             raise ValueError(f"{N} prompt tokens exceed the {cap} slots of the full-KV store")
-        return self._layer_major(ids, kv_cache, chunk)
+        return self._layer_major(ids, kv_cache, chunk, targets=targets, logprobs=logprobs)
 
     def extend(self, input_ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int = 128,
-               queries: Optional[torch.Tensor] = None) -> torch.Tensor:
+               queries: Optional[torch.Tensor] = None, logprobs=None) -> torch.Tensor:
         """Append n prompt rows after the store's `seq_len` rows (a follow-up turn over a prefilled context); returns the logits
         of the last row, [1, 1, V].  `queries`: None, or [L, H, d] fp16 that receives each layer's post-RoPE query of the last
         row (what the retrieval cache scores chunks with, RetrievalCache.reselect).
@@ -499,7 +536,8 @@ class LlamaModel:
         An E4M3 store or E4M3 weights: layer-major, like `prefill` (each layer's weights dequantized once per call).  Over a
         non-empty E4M3 store each piece appends its rows with the E4M3 RoPE kernel and attends over the store: pieces of more than
         64 rows on the causal wgmma kernel at head_dim 128 (tf_tree_attn_tc_causal_e4m3), others on the E4M3 verify attention.
-        Over an empty store the call is `prefill`."""
+        Over an empty store the call is `prefill`.  `logprobs`: the scores of ids[1:] given the store's rows and the ids before
+        them, as in `prefill`."""
         ids = input_ids.reshape(-1)
         N, start = ids.numel(), kv_cache.seq_len
         if N < 1:
@@ -508,17 +546,20 @@ class LlamaModel:
             raise ValueError(f"appending {N} tokens after {start} exceeds the {kv_cache.slots} slots of the full-KV store")
         if queries is not None:
             assert queries.dtype == torch.float16 and queries.shape == (len(self.layers), self.local_num_heads, self.head_dim)
+        targets = self._score_targets(ids, logprobs)
         if kv_dtype_of(kv_cache) == "fp16" and self.weight_dtype == "fp16":
             for c0 in range(0, N, chunk):
                 logits = self.forward_target(ids[c0:c0 + chunk], kv_cache, queries=queries if c0 + chunk >= N else None)
+                self._score_piece(logits[0], c0, targets, logprobs)
         else:
-            logits = self._layer_major(ids, kv_cache, chunk, queries)
+            logits = self._layer_major(ids, kv_cache, chunk, queries, targets=targets, logprobs=logprobs)
         return logits[:, -1:]
 
     def _layer_major(self, ids: torch.Tensor, kv_cache: FlashSimpleCache, chunk: int,
-                     queries: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     queries: Optional[torch.Tensor] = None, targets: Optional[torch.Tensor] = None, logprobs=None) -> torch.Tensor:
         """The N ids after the store's seq_len rows, layer by layer in `chunk`-id pieces (see `prefill` and `extend`); the
-        caller has checked the capacity.  An empty E4M3 store takes the fp16 scratch of `prefill`."""
+        caller has checked the capacity.  An empty E4M3 store takes the fp16 scratch of `prefill`.  `targets` (from
+        `_score_targets`): the head also runs on every piece but the last, in turn, into x and one piece of logits."""
         start = kv_cache.seq_len
         e4m3_store = kv_dtype_of(kv_cache) == "e4m3"
         scratch = e4m3_store and start == 0
@@ -568,7 +609,11 @@ class LlamaModel:
             del scratch_k, scratch_v
         del maps
         c0 = (N - 1) // chunk * chunk
+        if targets is not None:
+            for i, p0 in enumerate(range(0, c0, chunk)):
+                self._score_piece(self._head(h[p0:p0 + chunk], delta[i], x), p0, targets, logprobs)
         logits = self._head(h[c0:], delta[-1], x[:N - c0])
+        self._score_piece(logits, c0, targets, logprobs)
         kv_cache.seq_len = start + N
         return logits.unsqueeze(0)
 

@@ -732,6 +732,31 @@ def sample_argmax(probs: torch.Tensor, expo: torch.Tensor, out: Optional[torch.T
     return out
 
 
+def token_logprobs(logits: torch.Tensor, ids: torch.Tensor, logprob: Optional[torch.Tensor] = None,
+                   argmax: Optional[torch.Tensor] = None, check_ids: bool = True):
+    """tf_token_logprobs: (logprob fp32 [rows], argmax int32 [rows]) of the int32 ids [rows] under the fp32 logits rows
+    [rows, V] (row stride free, unit column stride).  The ids are checked to lie in [0, V) first (one device sync); a caller
+    that has checked them already passes check_ids=False, which also makes the call capturable in a CUDA graph."""
+    require_cuda(logits, ids)
+    assert logits.dim() == 2 and logits.dtype == torch.float32 and logits.stride(1) == 1
+    rows, V = logits.shape
+    assert ids.dtype == torch.int32 and ids.shape == (rows,) and ids.is_contiguous()
+    if check_ids and rows:
+        lo, hi = (int(v) for v in torch.aminmax(ids))
+        if lo < 0 or hi >= V:
+            raise ValueError(f"token ids must lie in [0, {V}); got ids in [{lo}, {hi}]")
+    if logprob is None:
+        logprob = torch.empty(rows, dtype=torch.float32, device=logits.device)
+    if argmax is None:
+        argmax = torch.empty(rows, dtype=torch.int32, device=logits.device)
+    assert logprob.dtype == torch.float32 and argmax.dtype == torch.int32 and logprob.shape == argmax.shape == (rows,)
+    assert logprob.is_contiguous() and argmax.is_contiguous()
+    check(lib().tf_token_logprobs(logits.data_ptr(), logits.stride(0) if rows > 1 else V, rows, V, ids.data_ptr(),
+                                  logprob.data_ptr(), argmax.data_ptr(), stream_ptr()), "tf_token_logprobs")
+    COUNTER.n += 1
+    return logprob, argmax
+
+
 def residual_probs(p: torch.Tensor, q: torch.Tensor) -> torch.Tensor:
     out = torch.empty_like(p)
     check(lib().tf_residual_probs(p.data_ptr(), q.data_ptr(), p.shape[-1], out.data_ptr(), stream_ptr()), "tf_residual_probs")

@@ -8,6 +8,9 @@ prefilling it again.  `Session` runs the chain path (`GraphInferenceEngine`: dra
     s.append(next_question_ids)                   # extend the full KV, re-select the retrieval cache, feed the draft
     answer2 = s.generate(256, temperature=0.6, top_p=0.9, seed=1)
     s.truncate(n); s.append(other_question_ids)   # roll back to a saved length and ask something else
+    sc = s.score(candidate_answer_ids)            # log p(each id | context, earlier ids); the session does not change
+
+`score` runs between turns and leaves no trace: see `_Turns.score`.
 
 A turn is prefill or append followed by one generate.  The turn's first token is drawn when generate starts, from the logits
 prefill or append left, because that is where the turn's temperature, top_p and seed are given; the events and draws are those
@@ -28,9 +31,20 @@ from .sampling import norm_logits
 from .spectree import SpecTree, load_grow_map
 
 
+@dataclass
+class Score:
+    """What `score(ids)` returns, one entry per id, on the model's device: `logprobs` (fp32), log p(ids[i] | context, ids[:i])
+    under the model's own distribution (temperature 1, no top-p); `argmax` (int32), the id greedy decoding would emit there
+    (torch.argmax's rule); `greedy` (bool), argmax == ids."""
+    logprobs: torch.Tensor
+    argmax: torch.Tensor
+    greedy: torch.Tensor
+
+
 class _Turns:
     """The turn bookkeeping both sessions share: the committed ids, the pending token, the logits a turn starts from, the order
-    of calls and the rollback of the full KV's length.  A subclass sets `_kv` (the full-KV cache)."""
+    of calls, the rollback of the full KV's length and `score`.  A subclass sets `_kv` (the full-KV cache), `_model` (the
+    target), `_positions` (its RoPE positions) and `_score_extend` (its LlamaModel.extend call)."""
 
     def __init__(self):
         self.ids: List[int] = []            # the ids whose K/V rows the full KV holds, in order
@@ -43,9 +57,64 @@ class _Turns:
         raise NotImplementedError
 
     @property
+    def _model(self):
+        raise NotImplementedError
+
+    @property
+    def _positions(self) -> int:
+        return self._model.config.max_position_embeddings
+
+    def _score_extend(self, ids: torch.Tensor, logprobs) -> None:
+        raise NotImplementedError
+
+    @property
     def length(self) -> int:
         """The committed length: tokens in the full KV."""
         return self._kv.seq_len
+
+    @torch.inference_mode()
+    def score(self, ids) -> Score:
+        """Score `ids` as a continuation of the committed context: the first id on the row the next token would be drawn from
+        (the held logits of prefill or append, or the pending token's row, which is forwarded first), each later id on the row
+        of the id before it.  The rows go into the full KV after its committed length (LlamaModel.extend with `logprobs`) and
+        the length is rolled back: the ids, the pending token, the turn's logits, the retrieval cache, the draft and the
+        captured graphs are as they were.  Refused, before anything changes, before prefill, after a truncate (no row to
+        condition on) and past the full KV's slots or the model's RoPE positions."""
+        if not self.ids:
+            raise RuntimeError("score before prefill: the session has no context")
+        if self.pending is None:
+            self._check_turn()
+        new = [int(i) for i in _as_ids(ids)[0].tolist()]
+        if not new:
+            raise ValueError("score needs at least one id")
+        m = self._model
+        V = m.config.vocab_size
+        if not all(0 <= i < V for i in new):
+            raise ValueError(f"token ids must lie in [0, {V}); got ids in [{min(new)}, {max(new)}]")
+        # rows forwarded: the pending token and every id (the last id's row is forwarded too: extend scores within its ids)
+        rows = [self.pending] + new if self.pending is not None else new
+        kv = self._kv
+        if len(rows) > 1:
+            if kv.seq_len + len(rows) > kv.slots:
+                raise ValueError(f"appending {len(rows)} tokens after {kv.seq_len} exceeds the {kv.slots} slots of the full-KV store")
+            if kv.seq_len + len(rows) > self._positions:
+                raise ValueError(f"appending {len(rows)} tokens after {kv.seq_len} reaches past the model's "
+                                 f"{self._positions} RoPE positions")
+        n = len(new)
+        target = torch.tensor(new, dtype=torch.int32, device=m.device)
+        lp = torch.empty(n, dtype=torch.float32, device=m.device)
+        am = torch.empty(n, dtype=torch.int32, device=m.device)
+        k = 0
+        if self.pending is None:  # the first id on the held last-row logits
+            ops.token_logprobs(self._logits.reshape(-1, V)[-1:], target[:1], lp[:1], am[:1], check_ids=False)
+            k = 1
+        if len(rows) > 1:
+            start = kv.seq_len
+            try:
+                self._score_extend(torch.tensor([rows], dtype=torch.int64, device=m.device), (lp[k:], am[k:]))
+            finally:
+                kv.seq_len = start  # extend moved only the host length; the device copy the graphs read is untouched
+        return Score(logprobs=lp, argmax=am, greedy=am == target)
 
     def _new_ids(self, ids, keep_pending: bool) -> List[int]:
         """The ids an append forwards: the pending token (if kept) and `ids`."""
@@ -98,6 +167,13 @@ class Session(_Turns):
     @property
     def _kv(self):
         return self.eng.kv_cache
+
+    @property
+    def _model(self):
+        return self.eng.model
+
+    def _score_extend(self, ids: torch.Tensor, logprobs) -> None:
+        self.eng.model.extend(ids, self.eng.kv_cache, chunk=self.eng.target_prefill_chunk, logprobs=logprobs)
 
     @torch.inference_mode()
     def prefill(self, ids) -> None:
@@ -255,12 +331,19 @@ class TreeSession(_Turns):
         return self.llm.kv_cache
 
     @property
+    def _model(self):
+        return self.llm.model
+
+    @property
     def _rc(self):
         return self.llm.retrieval_cache
 
     @property
     def _positions(self) -> int:
         return self.llm.config.max_position_embeddings
+
+    def _score_extend(self, ids: torch.Tensor, logprobs) -> None:
+        self.llm.model.extend(ids, self._kv, logprobs=logprobs)
 
     def _tree(self, temperature: float, top_p: float) -> SpecTree:
         key = (float(temperature), float(top_p))
