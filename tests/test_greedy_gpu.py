@@ -309,12 +309,12 @@ def _tokens_per_step(run):
     return (len(run.generated) - 1) / steps
 
 
-def _tiny_engine(alpha=TINY_ALPHA):
+def _tiny_engine(alpha=TINY_ALPHA, budget=None):
     ts, ds = named_config(TINY["target"]), named_config(TINY["draft"])
     target = LlamaModel(ts, numpy_state_dict(ts, TINY["target_seed"]), device=DEV)
     draft = LlamaModel(ds, numpy_state_dict(ds, TINY["draft_seed"]), device=DEV, is_draft=True)
     retune_agreement(target, draft, alpha, alpha, {})
-    P, B, c, g = TINY["prefill"], TINY["budget"], TINY["chunk"], TINY["gamma"]
+    P, B, c, g = TINY["prefill"], budget or TINY["budget"], TINY["chunk"], TINY["gamma"]
     cache = FlashSimpleCache(target, P + 256)
     graph_cache = RetrievalCache(target, max_budget=B, prefill=P, gamma=g, chunk_size=c)
     draft_cache = StreamingLLMEvictionCache(draft, start_size=16, recent_size=256 - 16 - g, gamma=g)
@@ -338,8 +338,8 @@ def test_tiny_stepwise_loop_is_greedy_ar():
     assert tps > 1.0 and run.accepted_count > 0
 
 
-def test_tiny_device_loop_is_greedy_ar():
-    ge = _tiny_engine()
+def test_tiny_device_loop_with_a_128_row_tail_is_greedy_ar():
+    ge = _tiny_engine(budget=128)  # 96 generated tokens need a retrieval tail of more than the case's 64 rows
     ids = numpy_prompt(TINY["prefill"], seed=TINY["prompt_seed"]).cuda()
     gen = 96
     ar, ar_rows = greedy_ar(ge, ids, gen + 8)

@@ -217,11 +217,15 @@ __global__ void __launch_bounds__(256) tail_update_kernel(const __half* __restri
                                                           int prefill, int budget, int seq_len_host,
                                                           const int32_t* __restrict__ seq_len_dev) {
   const int h = blockIdx.y, layer = blockIdx.z;
-  const int n_new = seq_len_host + (seq_len_dev ? *seq_len_dev : 0) - prefill;
+  // rows [seq_len - n_new, seq_len) go to [budget - n_new, budget): never more than the budget, whatever length the device
+  // holds (the hosts refuse a step that would pass it; this keeps a wrong length from writing outside the budget)
+  const int seq_len = seq_len_host + (seq_len_dev ? *seq_len_dev : 0);
+  const int n_new = min(seq_len - prefill, budget);
   if (n_new <= 0) return;
+  const int src_row = seq_len - n_new;
   const int vec_per_row = D / 8;
   const int total = n_new * vec_per_row;
-  const size_t src0 = (size_t)layer * kls + (size_t)h * khs + (size_t)prefill * D;
+  const size_t src0 = (size_t)layer * kls + (size_t)h * khs + (size_t)src_row * D;
   const size_t dst0 = (size_t)layer * rls + (size_t)h * rhs + (size_t)(budget - n_new) * D;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const size_t off = (size_t)i * 8;
@@ -238,14 +242,17 @@ __global__ void __launch_bounds__(256) tail_update_e4m3_kernel(const uint8_t* __
                                                                int prefill, int budget, int seq_len_host,
                                                                const int32_t* __restrict__ seq_len_dev) {
   const int h = blockIdx.y, layer = blockIdx.z;
-  const int n_new = seq_len_host + (seq_len_dev ? *seq_len_dev : 0) - prefill;
+  // the rows of tail_update_kernel: the last min(seq_len - prefill, budget), never outside the budget
+  const int seq_len = seq_len_host + (seq_len_dev ? *seq_len_dev : 0);
+  const int n_new = min(seq_len - prefill, budget);
   if (n_new <= 0) return;
+  const int src_row = seq_len - n_new;
   const int vec_per_row = D / 8;
   const int total = n_new * vec_per_row;
   const size_t head = (size_t)layer * kls + (size_t)h * khs;
   const size_t dst0 = (size_t)layer * rls + (size_t)h * rhs + (size_t)(budget - n_new) * D;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const size_t slot = (size_t)prefill + i / vec_per_row;
+    const size_t slot = (size_t)src_row + i / vec_per_row;
     const size_t src = head + slot * D + (size_t)(i % vec_per_row) * 8;
     const size_t ex = head / D + slot;
     *reinterpret_cast<uint4*>(rK + dst0 + (size_t)i * 8) = kv_e4m3_dequant8(*reinterpret_cast<const uint2*>(K + src), Ke[ex]);
@@ -263,9 +270,12 @@ __global__ void __launch_bounds__(256) tail_update_to_e4m3_kernel(const void* __
                                                                   int8_t* __restrict__ rVe, long long rls, long long rhs, int prefill,
                                                                   int budget, int seq_len_host, const int32_t* __restrict__ seq_len_dev) {
   const int h = blockIdx.y, layer = blockIdx.z, lane = threadIdx.x & 31;
-  const int n_new = seq_len_host + (seq_len_dev ? *seq_len_dev : 0) - prefill;
+  // the rows of tail_update_kernel: the last min(seq_len - prefill, budget), never outside the budget
+  const int seq_len = seq_len_host + (seq_len_dev ? *seq_len_dev : 0);
+  const int n_new = min(seq_len - prefill, budget);
   if (n_new <= 0) return;
-  const size_t src0 = ((size_t)layer * kls + (size_t)h * khs) / D + prefill;
+  const int src_row = seq_len - n_new;
+  const size_t src0 = ((size_t)layer * kls + (size_t)h * khs) / D + src_row;
   const size_t dst0 = ((size_t)layer * rls + (size_t)h * rhs) / D + (budget - n_new);
   for (int r = blockIdx.x * 8 + (threadIdx.x >> 5); r < n_new; r += gridDim.x * 8) {
     kv_e4m3_row_into<D, SRC_E4M3>(K, Ke, src0 + r, rK, rKe, dst0 + r, lane);

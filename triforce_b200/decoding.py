@@ -151,9 +151,39 @@ def prompt_phase(graph_engine, input_ids, trace=None, skip_target_prefill: bool 
     return logits
 
 
+def chain_room(eng, gamma: int) -> Optional[str]:
+    """None when the next chain step fits its caches, else the limit it would pass.  From the committed length S a step
+    writes at most gamma + 2 full-KV rows (the device loop always pads its verify to gamma + 2), commits at most gamma + 2
+    rows, all of which the tail copy puts in the retrieval budget, and takes RoPE positions up to S + gamma + 1:
+    "slots" (the full-KV store), "tail" (the retrieval budget past its `prefill` boundary) or "positions" (the RoPE table)."""
+    kv, gc = eng.kv_cache, eng.graph_cache
+    end = kv.seq_len + gamma + 2
+    if end > kv.slots:
+        return "slots"
+    if end - gc.prefill > gc.max_budget:
+        return "tail"
+    if end > eng.model.config.max_position_embeddings:
+        return "positions"
+    return None
+
+
+def check_room(eng, gamma: int) -> None:
+    """Refuse, before anything changes, a chain step that `chain_room` says would not fit."""
+    stop = chain_room(eng, gamma)
+    if stop is None:
+        return
+    kv, gc, S = eng.kv_cache, eng.graph_cache, eng.kv_cache.seq_len
+    why = {"slots": f"past the {kv.slots} slots of the full-KV store",
+           "tail": f"past the retrieval budget of {gc.max_budget} rows after its boundary {gc.prefill}",
+           "positions": f"past the model's {eng.model.config.max_position_embeddings} RoPE positions"}[stop]
+    raise ValueError(f"no room for a step ({stop}): {S} committed tokens + up to {gamma + 2} rows of a gamma={gamma} step "
+                     f"reach {why}")
+
+
 class TriForceRun:
     """Step-wise form of `TriForce` (decoding.py:41-160): `prefill()` = :44-62, `step()` = one pass of the :70-141 loop.
-    `TriForce(...)` below drives it; `bench.py` drives it directly to time exactly K steps."""
+    `TriForce(...)` below drives it; `bench.py` drives it directly to time exactly K steps.  A step that would not fit the
+    caches (`chain_room`) is refused with a ValueError before anything changes; the reference fails inside its tail copy."""
 
     def __init__(self, tokenizer, graph_engine, gamma=4, top_k=-1, top_p=0.9, temperature=0.6, noise=None, trace=None,
                  strict_less=True, pad_full_verify: bool = False):
@@ -192,10 +222,14 @@ class TriForceRun:
         self.generated = [self.next_token]
         return self.next_token
 
+    def room(self) -> Optional[str]:
+        return chain_room(self.eng, self.gamma)
+
     @torch.inference_mode()
     def step(self) -> int:
         """One outer iteration; returns the number of tokens it produced."""
         eng, ge, buf, trace, noise, gamma = self.eng, self.ge, self.buf, self.trace, self.noise, self.gamma
+        check_room(eng, gamma)
         n_before = self.n
         next_token = self.next_token
         # speculative decoding for draft (68m) and retrieval 7b model

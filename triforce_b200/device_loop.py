@@ -240,8 +240,15 @@ class DeviceLoopRun:
         self.h2d_bytes += 8
         return tok
 
+    def room(self) -> Optional[str]:
+        from .decoding import chain_room
+        return chain_room(self.eng, self.gamma)
+
     @torch.inference_mode()
     def step(self) -> int:
+        """One graph launch; refused like `TriForceRun.step` when it would not fit the caches (decoding.chain_room)."""
+        from .decoding import check_room
+        check_room(self.eng, self.gamma)
         self.loop.launch()
         r, toks = self.loop.read()
         produced, count, rejected, g2, examined, hit_eos, inner, inner_acc, shift, new_len = r[:10]

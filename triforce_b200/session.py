@@ -162,6 +162,7 @@ class Session(_Turns):
         self.strict_less, self.pad_full_verify = strict_less, pad_full_verify
         super().__init__()
         self.last_run = None                # the TriForceRun / DeviceLoopRun of the last turn (its counts)
+        self.last_stop: Optional[str] = None  # why the last turn stopped (see generate)
         self._draft_stale = False
 
     @property
@@ -210,7 +211,9 @@ class Session(_Turns):
         """Draw the turn's first token, then run TriForce steps until at least `max_new` tokens: step-wise (decoding.TriForceRun)
         or one whole-loop graph launch per step (device_loop.DeviceLoopRun, re-captured when a re-selection moved the retrieval
         boundary).  Noise: the device Philox stream of `seed`, or for the step-wise loop any noise source (`noise`).  Returns
-        the turn's tokens; all but the last are committed, the last is pending."""
+        the turn's tokens; all but the last are committed, the last is pending.
+        The turn stops early, before a step that would not fit (decoding.chain_room), and `last_stop` says why: "max_new",
+        "slots", "tail" or "positions".  After "tail" an append re-selects the retrieval boundary and the next turn goes on."""
         self._check_turn()
         if device_loop:
             if noise is not None:
@@ -223,7 +226,12 @@ class Session(_Turns):
                               strict_less=self.strict_less, pad_full_verify=self.pad_full_verify)
         run.start(self._logits)
         self._logits = None
+        self.last_stop = "max_new"
         while run.n < max_new:
+            stop = run.room()
+            if stop is not None:
+                self.last_stop = stop
+                break
             run.step()
         self.ids += run.generated[:-1]
         self.pending = run.generated[-1]
